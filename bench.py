@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path of BASELINE.json on B200: ParoQuant INT4 linears of Llama-3-8B.
+"""bench.py -- the hot path of BASELINE.json: ParoQuant INT4 linears of Llama-3-8B.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--m 1]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--m 1] [--dump-outputs DIR]
 
 One "step" = one decode token through ALL quantised linears of Llama-3-8B (32 layers x
 {merged qkv 4096->6144 (3 rotations), o 4096->4096, merged gate_up 4096->28672 (2 rotations),
 down 14336->4096}) at batch M (default 1), bf16 activations, random-init weights in checkpoint
 format, prepacked once.  Attention / norms / sampling are outside the hot path and are not run;
 `value` is therefore decode tokens/s of the linear path, the part the reference's kernels own.
-Per step 3.66 GB of packed weights are streamed (>> 126 MB L2), so no L2 flush is needed.
+Per step 3.66 GB of packed weights are streamed (>> the H100's 50 MB L2), so no L2 flush is needed.
 
 N > 1 (torchrun, one rank per GPU): the same model tensor-parallel -- qkv / gate_up column-sharded
 (no communication), o / down row-sharded on 128-channel group boundaries + one NCCL all-reduce
@@ -16,6 +16,9 @@ each (strong scaling, as BASELINE.json config 5).
 
 `--impl reference`: the reference's arithmetic on the host cores (oracle/cpu_baseline.py; the
 reference itself is CUDA-only), a bounded sample per step.
+
+`--dump-outputs DIR`: after the timed steps, what the timed paths computed in their last step is written as float32
+DIR/<name>.npy (the inputs are seeded: the same arguments give the same inputs on every run).
 """
 from __future__ import annotations
 
@@ -45,32 +48,13 @@ SHAPES = {  # name: (K, part_sizes, kind)
 }
 
 
-def traffic_from_profile(kernel="decode"):
-    """DRAM bytes (read + write) of ONE launch of the dominant kernel, from the committed `ncu --set full` summaries:
-    decode_kernel on gate_up (61.29 MB algorithmic) or one stream_kernel chain launch (one block: 114.5 MB algorithmic)."""
-    f, what, alg = {
-        "decode": ("r02_decode_gate_up_m1_ncu.txt", "decode_kernel, gate_up 4096->28672 M=1", algorithmic_bytes(4096, [14336, 14336], 1)),
-        "chain": ("r02_chain_m1_ncu.txt", "stream_kernel, one chain launch (o, gate_up, down, qkv) M=1",
-                  sum(algorithmic_bytes(K, p, 1) for K, p, _ in SHAPES.values())),
-    }[kernel]
-    path = ROOT / "profiles" / f
-    if not path.exists():
-        return None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot = 0.0
-    for ln in path.read_text().splitlines():
-        t = ln.split()
-        if len(t) >= 3 and t[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and t[2] in unit:
-            tot += float(t[1].replace(",", "")) * unit[t[2]]
-    return {"bytes_per_launch": tot, "launch": what, "algorithmic_bytes": alg, "source": f"profiles/{f}"} if tot else None
-
-
 def measured_peaks():
+    """HBM GB/s and dense bf16 TFLOP/s: MEASURED_PEAKS.json where the machine provides one, else the H100 SXM data sheet."""
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 1590.0)), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 989.0)), "measured"
+    return 3350.0, 989.0, "h100_sxm_datasheet"
 
 
 def algorithmic_bytes(K, parts, M, G=128, R=8):
@@ -306,6 +290,9 @@ def run_ours(args):
     sampler.start()
     ms, run_step, final = timed_graph(torch, token, args.steps, args.warmup, barrier, use_graph)
     launches_per_step = model.launches
+    dumps = {}
+    if args.dump_outputs:   # the timed path's result of its last step, before anything else runs on these buffers
+        dumps["chain_residual_out" if model.chained else "tp_down_out"] = final.float().cpu().numpy()
     _log(f"timed region done: {ms:.3f} ms/step")
     t_end = time.time() + 0.6   # keep the identical load running briefly so the NVML sampler sees clocks under this workload
     while time.time() < t_end:
@@ -336,12 +323,14 @@ def run_ours(args):
     chain_launches = launches_per_step
     if world == 1 and not args.no_per_linear:
         ms_l, run_l, final_l = timed_graph(torch, model.token_linear, args.steps, args.warmup, barrier, use_graph)
+        if args.dump_outputs:
+            dumps["per_linear_down_out"] = final_l.float().cpu().numpy()
         per_linear = {"tokens_per_s": M * 1e3 / ms_l, "ms_per_step": ms_l, "launches_per_step": model.launches,
                       "api": "ParoLinearKernel.__call__ -> torch.ops.paro.linear (the call ParoQuantLinearMethod.apply makes), one launch per "
                              "linear, activations chained by slices, vLLM's norm / activation kernels not run"}
 
     if per_linear is not None:
-        ms_n, _, _ = timed_graph(torch, model.token_linear_with_neighbours, max(args.steps // 2, 5), 3, barrier, use_graph)
+        ms_n, _, _ = timed_graph(torch, model.token_linear_with_neighbours, args.steps, args.warmup, barrier, use_graph)
         per_linear["with_neighbour_kernels"] = {"tokens_per_s": M * 1e3 / ms_n, "ms_per_step": ms_n,
                                                  "what": "the same 128 launches + torch's rms_norm / silu*mul / residual-add kernels between them: "
                                                          "the work one chain launch per block does"}
@@ -390,13 +379,13 @@ def run_ours(args):
             "config": {"workload": f"Llama-3-8B all quantised linears, decode batch {M}: {LAYERS} x (qkv 4096->6144 P=3, o 4096->4096, "
                                    f"gate_up 4096->28672 P=2, down 14336->4096), INT4 g128 krot8, fused rotate+dequant+GEMV, activations chained",
                        "batch": M, "parallelism": f"tp{world}", "launch": "cuda_graph+pdl" if use_graph else "eager+pdl", "path": path,
-                       "l2": "3.66 GB of weights streamed per step >> 126 MB L2, no flush needed"},
+                       "l2": "3.66 GB of weights streamed per step >> 50 MB L2, no flush needed"},
             "e2e": {"value": M * 1e3 / ms_e2e, "unit": "tokens/s", "h2d_bytes_per_step": model.x_host.numel() * 2, "d2h_bytes_per_step": model.y_host.numel() * 2,
                     "api": "paroquant_b200.chain.ParoChain.__call__ + ParoLinearKernel.forward_into" if model.chained else "ParoLinearKernel.forward_into + dist.all_reduce"},
             "gpu_launches": launches_per_step * args.steps,
             "clocks": sampler.summary(),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                         "traffic": traffic_from_profile("chain"), "peak_source": src, "kernel": "paro::stream_kernel", "launches_per_step": launches_per_step,
+                         "peak_source": src, "kernel": "paro::stream_kernel", "launches_per_step": launches_per_step,
                          "algorithmic_bytes_per_step": step_bytes, "avg_launch_us": ms * 1e3 / max(launches_per_step, 1)},
         }
         line["config"]["headline_path"] = headline
@@ -410,7 +399,6 @@ def run_ours(args):
             line["config"]["path"] = "128 launches, one per (merged) linear, through torch.ops.paro.linear; activations chained by slices"
             line["e2e"]["api"] = "ParoLinearKernel.__call__ -> torch.ops.paro.linear"
             line["roofline"]["kernel"] = "paro::decode_kernel"
-            line["roofline"]["traffic"] = traffic_from_profile("decode")
         if world == 1 and not args.no_ref_gpu:
             line["vs_reference_gpu"] = reference_gpu_section(M, line["value"], per_linear)
         if world == 1 and not args.no_prefill:
@@ -423,6 +411,12 @@ def run_ours(args):
                 line["training_op"] = {"unavailable": repr(e)[:200]}
         if world == 1 and not args.no_cpu_baseline:
             line["cpu_baseline"] = cpu_baseline_sample(M)
+        if args.dump_outputs:
+            import numpy as np
+            out_dir = Path(args.dump_outputs)
+            out_dir.mkdir(parents=True, exist_ok=True)
+            for name, arr in dumps.items():
+                np.save(out_dir / f"{name}.npy", arr)
         print(json.dumps(line), flush=True)
     if world > 1:
         # destroy_process_group() can block for minutes in the NCCL heartbeat monitor once torchrun's TCPStore
@@ -490,7 +484,7 @@ def training_op_section():
 
 
 def prefill_section(dev):
-    """BASELINE.json config 3 beside the decode headline: fused rotate + dequant + tcgen05 GEMM at batch 256 / 1024 / 4096 on the
+    """BASELINE.json config 3 beside the decode headline: fused rotate + dequant + wgmma GEMM at batch 256 / 1024 / 4096 on the
     Llama-3-8B linear shapes plus the K = 11008 down projection, TFLOP/s against the measured bf16 tensor roofline (each call:
     rotation pre-pass + GEMM).  The headline figure is the 4096-token layer."""
     import torch
@@ -626,6 +620,7 @@ def main():
     ap.add_argument("--no-prefill", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true")
     ap.add_argument("--no-per-linear", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the timed paths' outputs of their last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * paro_b200.h -- C ABI of libparo_b200.so: the sm_100a (B200) implementation of ParoQuant's
+ * paro_b200.h -- C ABI of libparo_b200.so: the sm_90a (H100) implementation of ParoQuant's
  * hot path (scaled pairwise rotation of the activations + AWQ INT4 group dequant + GEMV/GEMM).
  *
  * Plain pointers and sizes only; no torch / ATen types.  Every pointer named "device" must be
@@ -134,7 +134,7 @@ size_t paro_workspace_bytes(const paro_linear_shape *shape, int64_t max_m);
  *   y          device [M, N] of shape->dtype
  *   workspace  device, >= paro_workspace_bytes(shape, M), 256-byte aligned
  * M <= 16 runs the fused rotate+dequant+GEMV kernel (HBM-bound); larger M the
- * rotate + tcgen05 GEMM path.                                                            */
+ * rotate + wgmma GEMM path.                                                            */
 int paro_linear_forward(const paro_linear_shape *shape, const void *packed, const void *x,
                         int64_t M, const void *bias, void *y, void *workspace,
                         size_t workspace_bytes, paro_stream_t stream);

@@ -2,13 +2,12 @@
 
     python oracle/build_ref.py
 
-Sources are compiled where they lie under /root/reference/paroquant/kernels/cuda/ (rotation.cu,
-rotation.cuh, pybind.cpp) -- nothing is copied into this repository.  The recipe is ours (torch's
-cpp_extension driving nvcc/ninja directly), with the compiler flags the reference's own loader
-passes (paroquant/kernels/cuda/__init__.py:30-41), for sm_100a.  Output:
-oracle/_ref/paroquant_rotation.so, git-ignored but shipped to the GPU box, where
-tools/gen_ref_golden.py and tests/test_gpu_reference.py load it with torch.ops.load_library in a
-separate process (it registers the same `rotation::rotate` op name as our own provider).
+Sources are compiled where they lie (REF: rotation.cu, rotation.cuh, pybind.cpp) -- nothing is copied into this
+repository.  The recipe is ours (torch's cpp_extension driving nvcc/ninja directly), with the compiler flags the
+reference's own loader passes (paroquant/kernels/cuda/__init__.py:30-41), for sm_90a.  Output:
+oracle/_ref/paroquant_rotation.so (git-ignored), which tools/ref_gpu.py loads with torch.ops.load_library in a
+separate process (it registers the same `rotation::rotate` op name as our own provider) to produce the golden data
+under tests/golden/ and the same-GPU baseline of bench.py.
 
 The GEMM half of the reference path is vLLM's Marlin, taken from the installed vllm wheel.
 """
@@ -28,7 +27,7 @@ def build() -> Path | None:
         return so
     if not REF.exists():
         return None  # GPU box: only the prebuilt file travels
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     from torch.utils.cpp_extension import load
 
     OUT.mkdir(exist_ok=True)

@@ -4,7 +4,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 ``--impl reference`` legs may import this module.  Nothing under ``paroquant_b200/`` does.
 
 Two independent restatements of the same algorithm live here and are checked against each other
-(tests/test_oracle.py) and against outputs of the unmodified reference kernels captured on a B200
+(tests/test_oracle.py) and against outputs of the unmodified reference kernels captured on an H100
 (tests/golden/ref_gpu_*.npz, made by tools/gen_ref_golden.py):
 
   * ``c_*``   -- thin ctypes wrappers over oracle/paro_oracle.c (scalar loops, ``fmaf``)

@@ -19,7 +19,7 @@
  * Parity pin: the reference ships no tests or golden vectors (SURVEY.md section 4), and its kernels
  * are CUDA-only, so they cannot execute in a GPU-less container.  The pin is therefore
  * tests/golden/ref_gpu_*.npz: outputs of the UNMODIFIED reference rotate kernel (compiled by
- * oracle/build_ref.py from the sources where they lie) and of vLLM's Marlin run on a B200 by
+ * oracle/build_ref.py from the sources where they lie) and of vLLM's Marlin run on an H100 by
  * tools/gen_ref_golden.py.  Until those fixtures exist this oracle is "parity unpinned".
  *
  * One documented deviation: the reference evaluates sin/cos with the GPU's MUFU approximations
@@ -152,7 +152,7 @@ void paro_oracle_awq_unpack(const int32_t *packed, int64_t rows, int64_t pcols, 
 /* ---------------------------------------------------------------- dequant
  * W[k][n] = T( (q[k][n] - z[k/G][n]) * s_T[k/G][n] ), returned as fp32 holding a T-representable
  * value.  (q - z) is exact in every T; the product is rounded once (SURVEY.md A.3, confirmed on
- * the B200 against Marlin with one-hot activations, see tests/golden/README.md).
+ * the H100 against Marlin with one-hot activations, see tests/golden/README.md).
  * For dtype == PARO_F32 the product is the plain fp32 product (mlx/load.py:46-54 math).
  * scales: [K/G][N] as T bit patterns (uint16) for half types, float for f32.            */
 void paro_oracle_dequant(const int32_t *qweight, const int32_t *qzeros, const void *scales,

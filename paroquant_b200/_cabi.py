@@ -133,7 +133,7 @@ def _need_cuda(*tensors) -> torch.device:
         if t is None:
             continue
         if not t.is_cuda:
-            raise RuntimeError("paroquant_b200 kernels are CUDA-only (sm_100a); got a CPU tensor")
+            raise RuntimeError("paroquant_b200 kernels are CUDA-only (sm_90a); got a CPU tensor")
         if dev is not None and t.device != dev:
             raise RuntimeError("all tensors must be on the same CUDA device")
         dev = t.device

@@ -1,4 +1,4 @@
-"""Ahead-of-time build of libparo_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+"""Ahead-of-time build of libparo_b200.so for sm_90a (nvcc cross-compiles without a GPU).
 
     python -m paroquant_b200.build [--force] [--verbose]
 
@@ -18,7 +18,7 @@ LIBDIR = ROOT / "lib"
 LIB = LIBDIR / "libparo_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     # the reference builds its kernel with --use_fast_math (kernels/cuda/__init__.py:30-40);
     # __sincosf / .ftz parity with it needs the same switch
     "--use_fast_math", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

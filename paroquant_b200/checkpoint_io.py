@@ -216,7 +216,7 @@ def load_paro_checkpoint(model_dir, *, modules_to_not_convert: list[str] | None 
         raise ValueError(f"{d}: quantization_config.quant_method is {qcfg.get('quant_method')!r}, expected 'paroquant'")
     bits, group, krot = int(qcfg.get("bits", 4)), int(qcfg.get("group_size", 128)), int(qcfg.get("krot", 8))
     if bits != 4 or group not in (64, 128):
-        raise ValueError(f"{d}: bits={bits}, group_size={group}: the B200 kernels implement INT4 with group_size 64 or 128 only")
+        raise ValueError(f"{d}: bits={bits}, group_size={group}: the kernels implement INT4 with group_size 64 or 128 only")
     quantized = find_quantized_modules(d)
     if modules_to_not_convert:
         quantized -= set(modules_to_not_convert)

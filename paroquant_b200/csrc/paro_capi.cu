@@ -1,6 +1,6 @@
 // extern "C" surface of libparo_b200.so (declared in include/paro_b200.h): argument checks with
 // the reference's error behaviour (TORCH_CHECK -> message, here: code + paro_last_error()),
-// dispatch to the sm_100a kernels.  No allocation, no host synchronisation.
+// dispatch to the sm_90a kernels.  No allocation, no host synchronisation.
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a ParoQuant kernels: dtype traits with the reference's
+// Shared device helpers for the sm_90a ParoQuant kernels: dtype traits with the reference's
 // rounding points, mbarrier / bulk-copy (TMA) / PDL PTX wrappers, error plumbing.
 #pragma once
 

@@ -3,29 +3,25 @@
 // rotate -> Marlin kernel pairs (/root/reference/paroquant/inference/backends/vllm/plugin.py:281-311).
 //
 // Formulation (operand-swapped, as the large-M kernel): D[n, m] += W[n, k] * x_rot[m, k]
-//   A = 128 output columns x 128 channels (one quantisation group) per ROUND, dequantised by CUDA cores
-//       straight into TENSOR MEMORY (tcgen05.st); thread = one output column = one TMEM lane.
+//   A = 128 output columns x 128 channels (one quantisation group) per ROUND, dequantised by CUDA cores straight
+//       into mma.sync A fragments (registers); warp = one 16-row tile of the block x one 64-channel half of every round.
 //   B = x_rot of the CTA's K-slice, 16 token rows (zero-padded), written once per CTA after the in-kernel
-//       rotation, UMMA K-major core-matrix order.
-//   D = fp32 [128 x 16] in TMEM, double buffered.  All rounds of a 128-column block accumulate into the
-//       SAME D whichever dequant set produced the A operand: the tensor core does the in-CTA part of the
-//       split-K reduction, and the result is read back ONCE per block (tcgen05.ld, one value per thread
-//       and token) -- no shared-memory exchange, no intra-CTA barrier in the main loop.
+//       rotation, K-major core-matrix order; read as mma.sync B fragments.
+//   D = fp32 [16 x 16] per warp in registers over all rounds of a 128-column block; at the block's end the two
+//       k-half warps of a tile add their partials through shared memory (fixed order) -- the in-CTA part of the
+//       split-K reduction.
 //
 // Work split: the `c` CTAs of a cluster cover K (ragged slices of whole groups); a cluster walks a range
 // of 128-column blocks of one partition.  Cross-slice partials are pushed through distributed shared
 // memory to rank (block mod c); one cluster barrier; fixed summation order (bit-reproducible).
 //
-// Roles (SETS x 4 dequant warps + 2): warps 0..4*SETS-1 workers (TMEM lane quarter = warp % 4): the
-// prologue rotates the slice's groups (tasks of one group x up to 4 token rows per warp, __syncwarp only);
-// the main loop takes rounds r = set, set + SETS, ...; the set that dequantised a block's last group reads
-// D back.  Warp 4*SETS:
-// TMA producer (ONE 8576-byte record = weights + scales + zeros of a round per cp.async.bulk, into an
-// mbarrier ring, issued before griddepcontrol.wait).  Warp 4*SETS+1: TMEM allocator + tcgen05.mma issuer
-// (one elected lane).
+// Roles (16 worker warps + 1): warps 0..15 workers (tile = warp % 8, k half = warp / 8): the prologue rotates the
+// slice's groups (tasks of one group x up to 4 token rows per warp, __syncwarp only); the main loop takes every
+// round.  Warp 16: TMA producer (ONE 8576-byte record = weights + scales + zeros of a round per cp.async.bulk, into
+// an mbarrier ring, issued before griddepcontrol.wait).
 //
 // Numerics: x_rot as paro_rotate.cu; W = T((q - z) * T(s)) with ONE rounding (the operand Marlin / AWQ
-// form); fp32 accumulation in TMEM; one rounding to T; bias added in T (plugin.py:309-310).
+// form); fp32 accumulation; one rounding to T; bias added in T (plugin.py:309-310).
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -35,15 +31,13 @@
 
 namespace paro {
 
-#ifndef PARO_DEC_UNROLL
-#define PARO_DEC_UNROLL 4
-#endif
-constexpr int kDecUnroll = PARO_DEC_UNROLL;   // chunks of the dequant loop unrolled per trip (4 = straight-line)
-
 constexpr int kDecMaxStages = 24;
-constexpr int kDecTmemCols = 512;
-constexpr int kDecN = 16;            // MMA N: token rows, zero-padded (M_mma = 128 needs N % 16 == 0)
+constexpr int kDecSets = 4;                     // worker warps = 4 x sets = 8 row tiles x 2 k halves
+constexpr int kDecWorkers = 4 * kDecSets;
+constexpr int kDecN = 16;            // B operand rows per group: token rows, zero-padded
 constexpr int kDecSmemLimit = 227 * 1024;
+constexpr int kDecBarBytes = 16 * kDecMaxStages + 256;   // ring barriers + the x-load barrier
+constexpr int kDecXchgBytes = 2 * 8 * 8 * 128;           // k-half partials: [2][8 tiles][8 values][32 lanes] fp32 (in the rotation tiles)
 // one record per ring stage: 8576 bytes (group_size 128) or 8960 (group_size 64), both multiples of 64 -> DecParams::rec_bytes
 
 constexpr int kDecTraceSlots = 12;
@@ -170,10 +164,10 @@ __device__ __forceinline__ void dec_store(const DecParams &p, float v, int m, in
   static_cast<T *>(p.y)[static_cast<int64_t>(m) * p.N + n] = t;
 }
 
-template <typename T, int SETS>
-__global__ void __launch_bounds__(32 * (4 * SETS + 2), 1) decode_kernel(const DecParams p) {
+template <typename T>
+__global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const DecParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
-  constexpr int kWorkers = 4 * SETS;
+  constexpr int kWorkers = kDecWorkers;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long t_entry = clock64();
   if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 10] = globaltimer_ns();
@@ -181,10 +175,9 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 2), 1) decode_kernel(const De
   const uint32_t smem0 = smem_u32(smem);
   const uint32_t xb = smem0 + p.xb_off, recv = smem0 + p.recv_off, bars = smem0 + p.bar_off;
   const uint32_t bar_wfull = bars, bar_wempty = bars + 8 * kDecMaxStages;
-  const uint32_t bar_afull = bars + 16 * kDecMaxStages, bar_afree = bar_afull + 64;
-  const uint32_t bar_dfull = bar_afull + 128, bar_dfree = bar_afull + 192, bar_xb = bar_afull + 208, tmem_slot = bar_afull + 216;
-  const uint32_t bar_xload = bar_afull + 224;   // pre-rotated x: one bulk copy fills the whole B operand
-  constexpr uint32_t d_col0 = 64 * SETS;
+  const uint32_t bar_xload = bars + 16 * kDecMaxStages;   // pre-rotated x: one bulk copy fills the whole B operand
+  // k-half partials, [block parity][tile][8 values][32 lanes] fp32: in the rotation tiles' space, free once the B operand is complete
+  const uint32_t xchg = smem0 + p.rot_off;
 
   // ---- my range of 128-column blocks (within one partition) and my K-slice (whole groups, ragged)
   const int range = blockIdx.x >> p.c_shift;
@@ -210,37 +203,18 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 2), 1) decode_kernel(const De
   DecRotMeta rm;
   const int nq = p.M > 4 ? (p.M + 3) >> 2 : 1, ntasks = ng * nq;   // rotation tasks: row blocks of 4 for M > 4
   if (warp < kWorkers && warp < ntasks && warp < p.rot_warps)
-    dec_fetch_meta(p, part, g_begin + warp / nq, lane, rm);   // flies during the barrier init / TMEM allocation
+    dec_fetch_meta(p, part, g_begin + warp / nq, lane, rm);   // flies during the barrier initialisation
 
   if (warp == kWorkers) {
-    // one barrier per lane
+    // one barrier per lane; every worker warp consumes every ring stage
     if (lane < NS) {
       mbar_init(bar_wfull + 8 * lane, 1);
-      mbar_init(bar_wempty + 8 * lane, 4);
+      mbar_init(bar_wempty + 8 * lane, kWorkers);
     }
-    // Every barrier has ONE waiting party that consumes its phases in order (a parity wait issued a phase early passes
-    // on the stale phase): A-buffer and D-ready barriers are per dequant set, ring stages are always consumed by the
-    // same set (stage count is a multiple of SETS), the producer / MMA lanes wait sequentially on the rest.
-    if (lane < SETS) {
-      mbar_init(bar_afull + 8 * lane, 4);
-      mbar_init(bar_afree + 8 * lane, 1);
-      mbar_init(bar_dfull + 8 * lane, 1);
-    }
-    if (lane < 2) mbar_init(bar_dfree + 8 * lane, 4);
-    if (lane == 0) {
-      mbar_init(bar_xb, kWorkers);
-      mbar_init(bar_xload, 1);
-    }
+    if (lane == 0) mbar_init(bar_xload, 1);
     fence_mbar_init();
   }
-  if (warp == kWorkers + 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kDecTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = lds32(tmem_slot);
   DEC_TRACE(1);
   if (p.c > 1) cluster_arrive_relaxed();   // #1 "this CTA runs" -- waited on before the first DSMEM push into a peer's receive buffer
   pdl_launch_dependents();                 // let the next linear in the stream start prefetching its weights
@@ -263,146 +237,93 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 2), 1) decode_kernel(const De
       if (++st == NS) { st = 0; ++it; }
       if (++gi == ng) { gi = 0; ++j; }
     }
-  } else if (warp == kWorkers + 1) {
-    // ================= MMA issuer.  The whole warp runs the loop (waits included) and ONE elected lane issues:
-    // inside an `elect.sync` region ptxas keeps descriptors and TMEM addresses in uniform registers; under a plain
-    // `lane == 0` branch every tcgen05.mma was wrapped in a divergence loop (~15 instructions, ~120 cycles per MMA,
-    // tools/mma_probe.cu) and the single issuing thread, not the tensor pipe, bounded the kernel.
-    const uint32_t idesc = instr_desc<T>(kDecN);
+  } else {
+    // ================= workers: warp = (16-row tile of the block, k half of every record)
+    const int wi = warp, tile = warp & 7, kh = warp >> 3;
     if (p.pre_rotated) {
       // the pre-pass (paro_rotate.cu, tiled for 16 rows) wrote x_rot in exactly the B-operand order of this kernel, zero padding
-      // rows included: the K-slice's groups are ONE contiguous range -> one bulk copy, no rotation tasks, no proxy fence
-      pdl_wait();   // ... written by the previous kernel in the stream
-      if (elect_one()) {
-        const uint32_t bytes = static_cast<uint32_t>(ng) * (kDecN * 256);
-        mbar_arrive_expect_tx(bar_xload, bytes);
-        bulk_g2s(xb, static_cast<const uint8_t *>(p.x) + (static_cast<size_t>(part) * p.x_part_stride + static_cast<size_t>(g_begin) * (kDecN * kGroup)) * 2,
-                 bytes, bar_xload, policy_evict_first());
+      // rows included: the K-slice's groups are ONE contiguous range -> one bulk copy, no rotation tasks
+      if (wi == 0) {
+        pdl_wait();   // ... written by the previous kernel in the stream
+        if (elect_one()) {
+          const uint32_t bytes = static_cast<uint32_t>(ng) * (kDecN * 256);
+          mbar_arrive_expect_tx(bar_xload, bytes);
+          bulk_g2s(xb, static_cast<const uint8_t *>(p.x) + (static_cast<size_t>(part) * p.x_part_stride + static_cast<size_t>(g_begin) * (kDecN * kGroup)) * 2,
+                   bytes, bar_xload, policy_evict_first());
+        }
+        __syncwarp();
       }
-      __syncwarp();
       mbar_wait(bar_xload, 0);
-    }
-    mbar_wait(bar_xb, 0);   // B operand rows written (generic proxy) and fenced by the workers
-    const uint64_t desc_hi = smem_desc_kmajor(0, kDecN * 16, 128);   // everything but the start address
-    int set = 0, use = 0, j = 0, gi = 0;
-#pragma unroll 1
-    for (int r = 0; r < nrounds; ++r) {
-      if (gi == 0 && j >= 2) mbar_wait(bar_dfree + 8 * (j & 1), ((j >> 1) - 1) & 1);   // D buffer read back by its previous user
-      mbar_wait(bar_afull + 8 * set, use & 1);
-      tc_fence_after();
-      const uint32_t td = tmem + d_col0 + (j & 1) * kDecN, ta = tmem + set * 64;
-      const uint64_t bdesc0 = desc_hi | static_cast<uint64_t>(((xb + gi * (kDecN * 256)) >> 4) & 0x3FFF);
-      if (elect_one()) {
-#pragma unroll
-        for (int s = 0; s < 8; ++s) tc_mma_ts(td, ta + 8 * s, bdesc0 + s * ((kDecN * 32) >> 4), idesc, (gi | s) ? 1u : 0u);
-        tc_commit(bar_afree + 8 * set);
-        if (gi == ng - 1) tc_commit(bar_dfull + 8 * set);   // the set that dequantised the block's last group reads D back
+    } else {
+      // rows [M, 16) of every group are the zero padding of the N = 16 MMA: all workers clear the B operand before the
+      // dependency wait (it does not depend on x); the rotation tasks then write only token rows
+      if (p.M < kDecN) {
+        for (int i = threadIdx.x; i < ng * (kDecN * 16); i += 32 * kWorkers) sts128u(xb + i * 16, make_uint4(0u, 0u, 0u, 0u));
+        named_bar_sync(1, 32 * kWorkers);
       }
-      __syncwarp();
-      if (++set == SETS) { set = 0; ++use; }
-      if (++gi == ng) { gi = 0; ++j; }
+      DEC_TRACE(2);
+      pdl_wait();  // x may have been written by the previous kernel
+      DEC_TRACE(3);
+      if (wi < ntasks && wi < p.rot_warps) {
+        const uint32_t rot = smem0 + p.rot_off + wi * p.rot_bytes;
+        const int M = p.M, rw = p.rot_warps;
+        if (M == 1) dec_prologue<T, 1>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
+        else if (M == 2) dec_prologue<T, 2>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
+        else dec_prologue<T, 4>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
+      }
+      named_bar_sync(2, 32 * kWorkers);   // B operand complete
     }
-  } else {
-    // ================= workers
-    const int wi = warp, e = wi >> 2, q = warp & 3;
-    const int L128 = 32 * q + lane;               // output column inside the 128-column block = TMEM lane
-    const uint32_t lane_base = static_cast<uint32_t>(32 * q) << 16;
-    // rows [M, 16) of every group are the zero padding of the N = 16 MMA: all workers clear the B operand before the
-    // dependency wait (it does not depend on x); the rotation tasks then write only token rows
-    if (p.M < kDecN && !p.pre_rotated) {
-      for (int i = threadIdx.x; i < ng * (kDecN * 16); i += 32 * kWorkers) sts128u(xb + i * 16, make_uint4(0u, 0u, 0u, 0u));
-      named_bar_sync(1, 32 * kWorkers);
-    }
-    DEC_TRACE(2);
-    if (!p.pre_rotated) pdl_wait();  // x may have been written by the previous kernel (pre-rotated: the MMA warp fetches it)
-    DEC_TRACE(3);
-    if (!p.pre_rotated && wi < ntasks && wi < p.rot_warps) {
-      const uint32_t rot = smem0 + p.rot_off + wi * p.rot_bytes;
-      const int M = p.M, rw = p.rot_warps;
-      if (M == 1) dec_prologue<T, 1>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
-      else if (M == 2) dec_prologue<T, 2>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
-      else dec_prologue<T, 4>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
-      fence_proxy_async_smem();  // B rows were written through the generic proxy, tcgen05.mma reads them through the async proxy
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_xb);
     DEC_TRACE(4);
 
     const int M = p.M;
-    int j = 0, gi = e;
-    while (gi >= ng && j < nj) { gi -= ng; ++j; }
-    int st = e, use = 0;
-    uint32_t par = 0, epi = 0;
-    const uint32_t ta = tmem + lane_base + e * 64;
-    const uint32_t col_off = (L128 >> 4) * 1024 + (L128 & 15) * 16;   // my 16-byte slots inside a record's weights
     const bool q2 = p.q2 != 0;
     const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
+    const int g = lane >> 2, t = lane & 3;
+    int st = 0;
+    uint32_t par = 0;
     bool first = true;
 #pragma unroll 1
-    for (int r = e; r < nrounds; r += SETS) {
-      mbar_wait(bar_wfull + 8 * st, par);
-      if (first) { DEC_TRACE(5); first = false; }
-      if (p.trace && q == 0 && lane == 0 && blockIdx.x == 0 && r < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * r + 1] = clock64() - t_entry;
-      const uint32_t rec = smem0 + st * rec_bytes;
-      RowDequant<T> dq;
-      dq.prep(lds16(rec + kBlockScaleOff + 2 * L128), lds8(rec + zero_off + L128));
-      uint32_t s_hi = 0, z_hi = 0;   // group_size 64: channels 64..127 of the record have their own scale / zero
-      if (q2) { s_hi = lds16(rec + kBlockScaleOff + 256 + 2 * L128); z_hi = lds8(rec + zero_off + 128 + L128); }
-      if (use > 0) mbar_wait(bar_afree + 8 * e, (use - 1) & 1);  // the MMAs of my previous round have drained my A buffer
-      tc_fence_after();
-      const uint32_t wbase = rec + col_off;
-#pragma unroll kDecUnroll
-      for (int c = 0; c < 4; ++c) {
-        const uint4 w4 = lds128(wbase + c * 256);
-        uint32_t regs[16];
-        if (c == 2 && q2) dq.prep(s_hi, z_hi);
-        dq.word(w4.x, regs + 0);
-        dq.word(w4.y, regs + 4);
-        dq.word(w4.z, regs + 8);
-        dq.word(w4.w, regs + 12);
-        tc_st16(ta + 16 * c, regs);
-      }
-      tc_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_afull + 8 * e);
-        mbar_arrive(bar_wempty + 8 * st);
-        if (p.trace && q == 0 && blockIdx.x == 0 && r < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * r + 2] = clock64() - t_entry;
-      }
-      if (gi == ng - 1) {
-        // ---- this set closed block j: read D back, one value per token
-        const int b = j & 1;
-        mbar_wait(bar_dfull + 8 * e, epi & 1);
-        ++epi;
-        tc_fence_after();
-        uint32_t v[16];
-        if (M <= 8) tc_ld8(tmem + lane_base + d_col0 + b * kDecN, v);
-        else tc_ld16(tmem + lane_base + d_col0 + b * kDecN, v);
-        tc_wait_ld();
-        tc_fence_before();
+    for (int j = 0; j < nj; ++j) {
+      float acc[2][4] = {};
+#pragma unroll 1
+      for (int gi = 0; gi < ng; ++gi) {
+        mbar_wait(bar_wfull + 8 * st, par);
+        if (first) { DEC_TRACE(5); first = false; }
+        const uint32_t rec = smem0 + st * rec_bytes, xbg = xb + gi * (kDecN * 256);
+        if (M > 8) mma_round<T, 2>(rec, q2, zero_off, xbg, kDecN, tile, kh, lane, acc);
+        else mma_round<T, 1>(rec, q2, zero_off, xbg, kDecN, tile, kh, lane, acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(bar_dfree + 8 * b);
-        if (p.c == 1) {
-          const int n = n_first + j * kBlockN + L128;
-          if (n < n_end) {
+        if (lane == 0) mbar_arrive(bar_wempty + 8 * st);
+        if (++st == NS) { st = 0; par ^= 1; }
+      }
+      // ---- block j closed: the k-half-1 warp hands its partial to its tile's k-half-0 warp, which adds it (fixed order)
+      // and stores or pushes the sum.  Two buffers by block parity: a warp writes buffer j & 1 again only after the pair
+      // barrier of block j + 1, which its partner reaches after reading it.
+      const uint32_t xc = xchg + ((j & 1) * 8 + tile) * (8 * 128) + lane * 4;
+      if (kh == 1) {
 #pragma unroll
-            for (int m = 0; m < 16; ++m)
-              if (m < M) dec_store<T>(p, __uint_as_float(v[m]), m, n);
+        for (int i = 0; i < 8; ++i) sts_f32(xc + i * 128, acc[i >> 2][i & 3]);
+      }
+      named_bar_sync(4 + tile, 64);
+      if (kh == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] += lds_f32(xc + i * 128);
+        if (p.c > 1 && !cluster_ready) { cluster_wait_acquire(); cluster_ready = true; }  // #1: every peer CTA is running
+        const uint32_t dst = p.c > 1 ? map_to_rank(recv + (((j >> p.c_shift) << p.c_shift) + slice) * (M * 512), j & (p.c - 1)) : 0u;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int col = 16 * tile + g + 8 * ((i >> 1) & 1), m = 8 * (i >> 2) + 2 * t + (i & 1);
+          if (m < M) {
+            const float v = acc[i >> 2][i & 3];
+            if (p.c == 1) {
+              const int n = n_first + j * kBlockN + col;
+              if (n < n_end) dec_store<T>(p, v, m, n);
+            } else {
+              st_cluster_f32(dst + m * 512 + col * 4, v);
+            }
           }
-        } else {
-          if (!cluster_ready) { cluster_wait_acquire(); cluster_ready = true; }  // #1: every peer CTA is running
-          const uint32_t dst = map_to_rank(recv + (((j >> p.c_shift) << p.c_shift) + slice) * (M * 512) + L128 * 4, j & (p.c - 1));
-#pragma unroll
-          for (int m = 0; m < 16; ++m)
-            if (m < M) st_cluster_f32(dst + m * 512, __uint_as_float(v[m]));
         }
       }
-      st += SETS;
-      if (st >= NS) { st -= NS; par ^= 1; }
-      ++use;
-      gi += SETS;
-      while (gi >= ng) { gi -= ng; ++j; }
     }
     DEC_TRACE(6);
   }
@@ -431,12 +352,6 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 2), 1) decode_kernel(const De
   }
   DEC_TRACE(8);
   if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 11] = globaltimer_ns();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWorkers + 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kDecTmemCols) : "memory");
-  }
 }
 
 int decode_trace_read(unsigned long long *host, int max_ctas) {
@@ -451,11 +366,10 @@ static int dec_env_int(const char *name, int dflt) {
   return v && *v ? atoi(v) : dflt;
 }
 // environment knobs are read ONCE per process (every launch used to pay half a dozen getenv calls)
-struct DecKnobs { int stages, no_cluster, force_c, verbose, no_pdl, trace, sets; };
+struct DecKnobs { int stages, no_cluster, force_c, verbose, no_pdl, trace; };
 static const DecKnobs &dec_knobs() {
   static const DecKnobs k = {dec_env_int("PARO_DECODE_STAGES", 0), dec_env_int("PARO_NO_CLUSTER", 0), dec_env_int("PARO_DECODE_C", 0),
-                             dec_env_int("PARO_DECODE_VERBOSE", 0), dec_env_int("PARO_NO_PDL", 0), dec_env_int("PARO_DECODE_TRACE", 0),
-                             dec_env_int("PARO_DECODE_SETS", 5)};
+                             dec_env_int("PARO_DECODE_VERBOSE", 0), dec_env_int("PARO_NO_PDL", 0), dec_env_int("PARO_DECODE_TRACE", 0)};
   return k;
 }
 
@@ -515,9 +429,9 @@ struct DecSmem { int xb_off, rot_off, recv_off, bar_off, nstages, rot_warps, tot
 
 static bool dec_carve_with(const DecPlan &plan, int M, int rot_bytes, int sets, int rot_warps, int stage_bytes, DecSmem &s) {
   const int xb_bytes = plan.ng_max * kDecN * 256;
-  const int rot_total = (rot_warps * rot_bytes + 127) / 128 * 128;
+  const int rot_total = rot_warps * rot_bytes > kDecXchgBytes ? (rot_warps * rot_bytes + 127) / 128 * 128 : kDecXchgBytes;
   const int recv = plan.c > 1 ? ((plan.nj_max + plan.c - 1) / plan.c) * plan.c * M * 512 : 0;
-  const int bar_bytes = 16 * kDecMaxStages + 256;
+  const int bar_bytes = kDecBarBytes;
   const int fixed = xb_bytes + rot_total + recv + bar_bytes + 128;
   int nst = (kDecSmemLimit - fixed) / stage_bytes;
   if (nst > kDecMaxStages) nst = kDecMaxStages;
@@ -547,16 +461,16 @@ static bool dec_carve(const DecPlan &plan, int M, int rot_bytes, int sets, int s
 }
 
 // how many clusters of `c` CTAs with this footprint the device keeps resident (GPC granularity); cached per thread
-template <typename T, int SETS>
+template <typename T>
 static int max_resident_clusters(int c, int smem_bytes, int sms) {
   if (c == 1) return sms;
   int slot = 0;
   while ((1 << slot) < c) ++slot;
-  auto kern = decode_kernel<T, SETS>;
+  auto kern = decode_kernel<T>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) { (void)cudaGetLastError(); return 0; }   // never lowered: cached plans keep launching
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((sms / c) * c);
-  cfg.blockDim = dim3(32 * (4 * SETS + 2));
+  cfg.blockDim = dim3(32 * (kDecWorkers + 1));
   cfg.dynamicSmemBytes = smem_bytes;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -624,9 +538,9 @@ int decode_debug_plan(const Layout &L, int64_t M, int sets, int sms, const int32
 
 struct DecCached { bool found; DecPlan plan; DecSmem smem; };
 
-template <typename T, int SETS>
+template <typename T>
 static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t stream) {
-  auto kern = decode_kernel<T, SETS>;
+  auto kern = decode_kernel<T>;
   const DecKnobs &kn = dec_knobs();
   // the plan (cluster size, block ranges, shared-memory carve-up) depends on the shape, M and the device only: searched once
   // (the search asks the occupancy API and sets the function attribute), then looked up -- an eager launch is a map lookup
@@ -647,8 +561,8 @@ static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t st
     auto it = cache.find(key);
     if (it == cache.end()) {
       DecCached fresh = {};
-      fresh.found = dec_choose_plan(L, p.M, p.rot_bytes, SETS, sms, !kn.no_cluster, kn.force_c,
-                                    [&](int cc, int smem) { return max_resident_clusters<T, SETS>(cc, smem, sms); }, fresh.plan, fresh.smem);
+      fresh.found = dec_choose_plan(L, p.M, p.rot_bytes, kDecSets, sms, !kn.no_cluster, kn.force_c,
+                                    [&](int cc, int smem) { return max_resident_clusters<T>(cc, smem, sms); }, fresh.plan, fresh.smem);
       if (fresh.found && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) {
         (void)cudaGetLastError();
         fresh.found = false;
@@ -666,7 +580,7 @@ static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t st
 
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(best.grid);
-  cfg.blockDim = dim3(32 * (4 * SETS + 2));
+  cfg.blockDim = dim3(32 * (kDecWorkers + 1));
   cfg.dynamicSmemBytes = best_s.total;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
@@ -753,14 +667,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   p.meta_group_bytes = L.meta_group_bytes;
   p.meta_off = static_cast<long long>(L.meta_off);
   p.rec_off = static_cast<long long>(L.rec_off);
-  const int sets = dec_knobs().sets;   // 5 sets x 4 dequant warps measured best (tools/microbench.py); 4..7 selectable
-  const bool bf16 = s.dtype == PARO_BF16;
-  switch (sets) {
-    case 4: return bf16 ? launch_decode<__nv_bfloat16, 4>(p, L, sms, stream) : launch_decode<__half, 4>(p, L, sms, stream);
-    case 7: return bf16 ? launch_decode<__nv_bfloat16, 7>(p, L, sms, stream) : launch_decode<__half, 7>(p, L, sms, stream);
-    case 6: return bf16 ? launch_decode<__nv_bfloat16, 6>(p, L, sms, stream) : launch_decode<__half, 6>(p, L, sms, stream);
-    default: return bf16 ? launch_decode<__nv_bfloat16, 5>(p, L, sms, stream) : launch_decode<__half, 5>(p, L, sms, stream);
-  }
+  return s.dtype == PARO_BF16 ? launch_decode<__nv_bfloat16>(p, L, sms, stream) : launch_decode<__half>(p, L, sms, stream);
 }
 
 }  // namespace paro

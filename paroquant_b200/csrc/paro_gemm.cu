@@ -1,21 +1,19 @@
-// Large-M path (M > 16): rotation pre-pass + INT4-dequant tcgen05 GEMM, tensor-core bound.
+// Large-M path (M > 16): rotation pre-pass + INT4-dequant wgmma GEMM, tensor-core bound.
 //
 //   y^T[n, m] = sum_k W[n, k] * x_rot[m, k]          (operand-swapped: the quantised weights are the
-//                                                      M_mma = 128 side, the tokens the N side)
-//   A  = W block of 128 output columns x 128 channels per round, dequantised by CUDA cores straight
-//        into TENSOR MEMORY (tcgen05.st): T((q - z) * T(s)), one rounding, the operand Marlin / AWQ form.
-//        No shared-memory round trip and no smem bandwidth spent on the weight operand.
+//                                                      M = 64 side of wgmma, the tokens the N side)
+//   A  = W block of 128 output columns x 128 channels per round, dequantised by the consumer warpgroups straight
+//        into wgmma's register A fragments: T((q - z) * T(s)), one rounding, the operand Marlin / AWQ form.
+//        No shared-memory round trip for the weight operand.
 //   B  = x_rot tile [NT tokens x 64 channels] per stage, produced by the rotation pre-pass
-//        (paro_rotate.cu, the reference's rounding points) directly in UMMA's K-major core-matrix
+//        (paro_rotate.cu, the reference's rounding points) directly in wgmma's K-major core-matrix
 //        order, so ONE 1-D bulk copy (TMA) per stage fills the operand -- no tensor map needed.
-//   D  = fp32 [128 x NT] in TMEM (NT <= 256 columns), one rounding to T in the epilogue, bias in T.
+//   D  = fp32 [64 x NT] per consumer warpgroup in registers, one rounding to T in the epilogue, bias in T.
 //
 // CTA = one (128-column block of N) x (NT-token block of M) output tile over the whole K.
-// Warp roles as in paro_decode.cu: warp 0 TMA producer (one 8576-byte weight record + 2 B stages per
-// round), warp 1 TMEM allocator + single-thread tcgen05.mma issuer, warps 2-17 four dequant sets
-// (thread = one output column; round r -> set r % 4, each set owns one A buffer), all of them read D back.
-// At NT = 256 one round is 8 MMAs x 128 cycles on the tensor pipe against ~260 dequant
-// instructions per worker thread: the CUDA cores idle, the tensor core does not.
+// Warpgroup 0: warp 0 TMA producer of the weight records (one 8576-byte record per round), warp 1 TMA producer of the
+// x_rot stages.  Warpgroups 1 and 2: consumers of output columns 0-63 / 64-127 of the block; a consumer dequantises
+// round r + 1 while the wgmmas of round r run (two register sets of A fragments).
 #include "paro_tc_common.cuh"
 
 namespace paro {
@@ -23,12 +21,10 @@ namespace paro {
 int rotate_small_launch(const void *x, void *out, const void *raw_base, long long raw_part_bytes, int n_parts, int64_t M, int64_t M_store, int nt,
                         int K, int krot, int dtype, cudaStream_t stream);
 
-constexpr int kGemmSets = 4;                       // dequant sets of 4 warps; round r -> set r % 4
-constexpr int kGemmThreads = 32 * (3 + 4 * kGemmSets);   // + weight producer, MMA issuer, x_rot producer
-constexpr int kGemmTmemCols = 512;
-constexpr int kWStages = 8;   // rounds of weights in flight (8 KB each); a multiple of kGemmSets
-constexpr int kBStages = 4;   // k64 stages of x_rot in flight (NT * 128 bytes each)
-constexpr int kABufs = kGemmSets;   // one A buffer (64 TMEM columns) per dequant set; D takes the other 256 columns
+constexpr int kGemmConsumers = 2;                         // warpgroups of 64 output columns
+constexpr int kGemmThreads = 128 * (1 + kGemmConsumers);
+constexpr int kWStages = 8;   // rounds of weights in flight (8.5 KB each)
+constexpr int kBStages = 4;   // k64 stages of x_rot in flight (NT * 128 bytes each): two rounds
 constexpr int kWStage = kBlockBytesMax;   // one (block, group) record per ring stage (8576 bytes, 8960 with group_size 64)
 
 struct GemmParams {
@@ -44,17 +40,31 @@ struct GemmParams {
   long long rec_off, xr_part_stride;
 };
 
+// the A fragments of one round (8 k16 steps x 4 registers) for this warp's rows r and r + 8
 template <typename T>
-__global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const GemmParams p) {
+__device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32_t zero_off, int r, int t, uint32_t (&a)[32]) {
+  RowDequant<T> d0, d1;
+  d0.prep(lds16(rec + kBlockScaleOff + 2 * r), lds8(rec + zero_off + r));
+  d1.prep(lds16(rec + kBlockScaleOff + 2 * (r + 8)), lds8(rec + zero_off + r + 8));
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    if (c == 2 && q2) {   // group_size 64: channels 64..127 of the record have their own scale / zero
+      d0.prep(lds16(rec + kBlockScaleOff + 256 + 2 * r), lds8(rec + zero_off + 128 + r));
+      d1.prep(lds16(rec + kBlockScaleOff + 256 + 2 * (r + 8)), lds8(rec + zero_off + 128 + r + 8));
+    }
+    frag_a2<T>(rec, r, c, t, d0, d1, *reinterpret_cast<uint32_t(*)[8]>(a + 8 * c));
+  }
+}
+
+template <typename T, int NT>
+__global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int NT = p.NT;
   const uint32_t smem0 = smem_u32(smem);
-  const uint32_t b_stage_bytes = NT * 128;
+  constexpr uint32_t b_stage_bytes = NT * 128;
   const uint32_t w_ring = smem0, b_ring = smem0 + kWStages * kWStage;
   const uint32_t bars = b_ring + kBStages * b_stage_bytes;
   const uint32_t bar_wfull = bars, bar_wempty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 160;
-  const uint32_t bar_afull = bars + 192, bar_afree = bars + 224, bar_dfull = bars + 256, tmem_slot = bars + 264;
 
   const int block = blockIdx.x % p.n_blocks, tb = blockIdx.x / p.n_blocks;   // 128-column block (over all partitions), token block
   int part = 0;
@@ -63,25 +73,15 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const GemmPara
   const int rounds = p.groups;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kWStages; ++s) { mbar_init(bar_wfull + 8 * s, 1); mbar_init(bar_wempty + 8 * s, 4); }
-    for (int s = 0; s < kBStages; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 1); }
-    for (int a = 0; a < kABufs; ++a) { mbar_init(bar_afull + 8 * a, 4); mbar_init(bar_afree + 8 * a, 1); }
-    mbar_init(bar_dfull, 1);
+    for (int s = 0; s < kWStages; ++s) { mbar_init(bar_wfull + 8 * s, 1); mbar_init(bar_wempty + 8 * s, 4 * kGemmConsumers); }
+    for (int s = 0; s < kBStages; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, kGemmConsumers); }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kGemmTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = lds32(tmem_slot);
-  const uint32_t d_col0 = 64 * kABufs;
 
   if (warp == 0) {
     // ================= weight producer: independent of the pre-pass; every 128-column block is re-read by
-    // all token blocks, so the units stay under the normal L2 policy (no evict-first here)
+    // all token blocks, so the records stay under the normal L2 policy (no evict-first here)
     if (lane == 0) {
       const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
       const uint8_t *rec = p.packed + p.rec_off + static_cast<size_t>(block) * p.groups * rec_bytes;
@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const GemmPara
                      : "memory");
       }
     }
-  } else if (warp == kGemmThreads / 32 - 1) {
+  } else if (warp == 1) {
     // ================= x_rot producer: one contiguous NT x 64 operand tile per stage
     if (lane == 0) {
       const uint8_t *xr_tile = p.xr + static_cast<size_t>(part) * p.xr_part_stride +
@@ -110,139 +110,112 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const GemmPara
                      : "memory");
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer: the whole warp runs the loop, ONE elected lane issues (inside an elect.sync
-    // region ptxas keeps descriptors in uniform registers; a plain `lane == 0` branch wraps every tcgen05.mma
-    // in a divergence loop and the issuing thread, not the tensor pipe, becomes the limit at small NT)
-    {
-      const uint32_t idesc = instr_desc<T>(NT);
-      const uint32_t step_bytes = NT * 32, lbo = NT * 16;
-      const uint64_t desc_hi = smem_desc_kmajor(0, lbo, 128);
-      int abuf = 0, a_use = 0;   // A buffer of round r = its dequant set = r % kGemmSets, r / kGemmSets earlier uses
-      for (int r = 0; r < rounds; ++r) {
-        mbar_wait(bar_afull + 8 * abuf, a_use & 1);
-        for (int hstage = 0; hstage < 2; ++hstage) {
-          const int bi = 2 * r + hstage, bs = bi % kBStages;
-          mbar_wait(bar_bfull + 8 * bs, (bi / kBStages) & 1);
-          tc_fence_after();
-          const uint64_t bdesc0 = desc_hi | static_cast<uint64_t>(((b_ring + bs * b_stage_bytes) >> 4) & 0x3FFF);
-          if (elect_one()) {
-#pragma unroll
-            for (int s4 = 0; s4 < 4; ++s4) {
-              const int s = hstage * 4 + s4;
-              tc_mma_ts(tmem + d_col0, tmem + abuf * 64 + 8 * s, bdesc0 + s4 * (step_bytes >> 4), idesc, (r | s) ? 1u : 0u);
-            }
-            tc_commit(bar_bempty + 8 * bs);
-            if (hstage == 1) {
-              tc_commit(bar_afree + 8 * abuf);
-              if (r == rounds - 1) tc_commit(bar_dfull);
-            }
-          }
-          __syncwarp();
-        }
-        if (++abuf == kABufs) { abuf = 0; ++a_use; }
-      }
-    }
-  } else {
-    // ================= workers: thread = one output column (TMEM lane)
-    const int wi = warp - 2, e = wi >> 2, q = warp & 3;
-    const int L128 = 32 * q + lane;                // column inside the 128-column block = TMEM lane
-    const uint32_t lane_base = static_cast<uint32_t>(32 * q) << 16;
-    const uint32_t col_off = (L128 >> 4) * 1024 + (L128 & 15) * 16;   // my 16-byte slots inside a record's weights
-    // Every barrier has ONE waiting party per phase sequence (set e waits only on its own A buffer's barriers): with
-    // A buffers shared between sets, a fast set could ask for a phase two ahead of the barrier and the parity test
-    // passes on the stale phase (seen as a hang / wrong results once the weight stream stopped pacing the workers).
-    const uint32_t ta = tmem + lane_base + e * 64;
+  } else if (warp >= 4) {
+    // ================= consumers: warpgroup wg owns output columns 64 wg .. 64 wg + 63 of the block
+    const int wg = (warp >> 2) - 1, w = warp & 3;
+    const int g = lane >> 2, t = lane & 3;
+    const int r = 64 * wg + 16 * w + g;   // my rows r and r + 8 inside the block
     const bool q2 = p.q2 != 0;
     const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
-    int use = 0;
-    for (int r = e; r < rounds; r += kGemmSets) {
-      const int ws = r % kWStages;
-      mbar_wait(bar_wfull + 8 * ws, (r / kWStages) & 1);
-      const uint32_t rec = w_ring + ws * kWStage;
-      RowDequant<T> dq;
-      dq.prep(lds16(rec + kBlockScaleOff + 2 * L128), lds8(rec + zero_off + L128));   // zero-filled past the partition's end
-      uint32_t s_hi = 0, z_hi = 0;   // group_size 64: channels 64..127 of the record have their own scale / zero
-      if (q2) { s_hi = lds16(rec + kBlockScaleOff + 256 + 2 * L128); z_hi = lds8(rec + zero_off + 128 + L128); }
-      if (use > 0) mbar_wait(bar_afree + 8 * e, (use - 1) & 1);
-      tc_fence_after();
-      const uint32_t wbase = rec + col_off;
+    const uint64_t desc_hi = smem_desc_kmajor(0, NT * 16, 128);
+    float acc[NT / 2];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const uint4 w4 = lds128(wbase + c * 256);
-        uint32_t regs[16];
-        if (c == 2 && q2) dq.prep(s_hi, z_hi);
-        dq.word(w4.x, regs + 0);
-        dq.word(w4.y, regs + 4);
-        dq.word(w4.z, regs + 8);
-        dq.word(w4.w, regs + 12);
-        tc_st16(ta + 16 * c, regs);
-      }
-      tc_wait_st();
-      tc_fence_before();
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    uint32_t a0[32], a1[32];
+
+    // dequantise round rr into `a` (the record's ring stage is released as soon as the fragments are in registers)
+    auto dequant = [&](int rr, uint32_t (&a)[32]) {
+      const int ws = rr % kWStages;
+      mbar_wait(bar_wfull + 8 * ws, (rr / kWStages) & 1);
+      gemm_dequant_round<T>(w_ring + ws * kWStage, q2, zero_off, r, t, a);
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_afull + 8 * e);
-        mbar_arrive(bar_wempty + 8 * ws);
+      if (lane == 0) mbar_arrive(bar_wempty + 8 * ws);
+    };
+    // issue the 8 wgmmas of round rr (B: its two x_rot stages), one commit group
+    auto issue = [&](int rr, const uint32_t (&a)[32]) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int bi = 2 * rr + h, bs = bi % kBStages;
+        mbar_wait(bar_bfull + 8 * bs, (bi / kBStages) & 1);
       }
-      ++use;
+      fence_operands(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int s = 0; s < 8; ++s) {
+        const int bs = (2 * rr + (s >> 2)) % kBStages;
+        const uint64_t desc = desc_hi | static_cast<uint64_t>(((b_ring + bs * b_stage_bytes + (s & 3) * (NT * 32)) >> 4) & 0x3FFF);
+        Wgmma<T, NT>::mma(acc, a + 4 * s, desc);
+      }
+      wgmma_commit();
+      fence_operands(acc);
+    };
+    // round rr's wgmmas have completed: its x_rot stages go back to the producer
+    auto release = [&](int rr) {
+      if (w == 0 && lane == 0) {
+        mbar_arrive(bar_bempty + 8 * ((2 * rr) % kBStages));
+        mbar_arrive(bar_bempty + 8 * ((2 * rr + 1) % kBStages));
+      }
+    };
+
+    dequant(0, a0);
+    for (int rr = 0; rr < rounds; rr += 2) {
+      issue(rr, a0);
+      if (rr + 1 < rounds) dequant(rr + 1, a1);
+      wgmma_wait<0>();
+      fence_operands(acc);
+      release(rr);
+      if (rr + 1 >= rounds) break;
+      issue(rr + 1, a1);
+      if (rr + 2 < rounds) dequant(rr + 2, a0);
+      wgmma_wait<0>();
+      fence_operands(acc);
+      release(rr + 1);
     }
 
-    // ---- epilogue: set e converts its share of the token columns of its lanes
-    mbar_wait(bar_dfull, 0);
-    tc_fence_after();
-    const int n = n0 + L128;
-    const bool n_ok = n < n_end;
-    float bias_f = 0.f;
-    const bool has_bias = p.bias != nullptr;
-    if (has_bias && n_ok) bias_f = Traits<T>::to_float(static_cast<const T *>(p.bias)[n]);
+    // ---- epilogue: acc[4j + e] = rows r (e < 2) / r + 8, tokens 8j + 2t + (e & 1)
     T *yout = static_cast<T *>(p.y);
-    const int set_cols = NT / kGemmSets >= 16 ? NT / kGemmSets : 16;   // token columns this set converts
-    for (int c0 = e * set_cols; c0 < (e + 1) * set_cols && c0 < NT; c0 += 16) {
-      uint32_t v[16];
-      tc_ld16(tmem + lane_base + d_col0 + c0, v);
-      tc_wait_ld();
+    const bool has_bias = p.bias != nullptr;
 #pragma unroll
-      for (int k = 0; k < 16; ++k) {
-        const int64_t m = static_cast<int64_t>(tb) * NT + c0 + k;
-        if (n_ok && m < p.M) {
-          T t = Traits<T>::from_float(__uint_as_float(v[k]));
-          if (has_bias) t = Traits<T>::from_float(Traits<T>::to_float(t) + bias_f);
-          yout[m * p.N + n] = t;
+    for (int hi = 0; hi < 2; ++hi) {
+      const int n = n0 + r + 8 * hi;
+      if (n >= n_end) continue;
+      const float bias_f = has_bias ? Traits<T>::to_float(static_cast<const T *>(p.bias)[n]) : 0.f;
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int64_t m = static_cast<int64_t>(tb) * NT + 8 * j + 2 * t + e;
+          if (m < p.M) {
+            T v = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
+            if (has_bias) v = Traits<T>::from_float(Traits<T>::to_float(v) + bias_f);
+            yout[m * p.N + n] = v;
+          }
         }
       }
     }
-  }
-
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kGemmTmemCols) : "memory");
   }
 }
 
 // ------------------------------------------------------------------ host side
-// Tokens per output tile.  The tensor pipe needs ~135 cycles per M128 x N256 x K16 MMA (8 per round), a dequant set ~520
-// cycles per round: N = 256 tiles keep the tensor pipe busy, but a small batch x few column blocks gives fewer tiles than SMs
-// (256 tokens x 4096 columns = 32 tiles) and is better cut finer -- pick the size with the shortest critical path
-// (waves x (rounds x max(dequant, MMA) + per-tile prologue / read-back)).
+// Tokens per output tile.  A round is 8 wgmmas of m64 x NT x k16 per consumer warpgroup (~NT * 8 tensor cycles for both) against
+// ~400 cycles of dequant per warpgroup: NT = 128 tiles keep the tensor pipe busy, but a small batch x few column blocks gives fewer
+// tiles than SMs (256 tokens x 4096 columns = 64 tiles) and is better cut finer -- pick the size with the shortest critical path
+// (waves x (rounds x max(dequant, MMA) + per-tile prologue / epilogue)).
 static int pick_nt(int64_t M, const Layout &L) {
   static int sms = 0;
   if (!sms) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
   }
   // from the largest tile the batch allows downwards: a finer tile must be CLEARLY better on paper (>= 25 %) -- finer tiles
   // re-read the weights more often and sit at the dequant limit, which the model prices optimistically
   int best = 0;
   double best_t = 0;
-  for (int nt = 256; nt >= 32; nt /= 2) {
+  for (int nt = 128; nt >= 32; nt /= 2) {
     if (nt > 32 && M <= nt / 2) continue;   // never pad the batch more than 2x
     const int64_t tiles = (M + nt - 1) / nt * L.blocks_total;
     const int64_t waves = (tiles + sms - 1) / sms;
-    const double per_round = nt * (8.0 * 135.0 / 256.0) > 520.0 ? nt * (8.0 * 135.0 / 256.0) : 520.0;
+    const double per_round = nt * 8.0 > 400.0 ? nt * 8.0 : 400.0;
     const double t = static_cast<double>(waves) * (L.groups * per_round + 4000.0 + 16.0 * nt);
     if (!best || t < 0.75 * best_t) { best = nt; best_t = t; }
   }
@@ -254,10 +227,10 @@ size_t gemm_workspace_bytes(const Layout &L, int64_t max_m) {
   return static_cast<size_t>(L.n_parts) * m_pad * L.K * 2;   // x_rot per partition, B-operand tile order
 }
 
-template <typename T>
+template <typename T, int NT>
 static int launch_gemm(const GemmParams &p, cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<T>;
-  const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * p.NT * 128 + 512;
+  auto kern = wg_gemm_kernel<T, NT>;
+  const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256;
   PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(p.n_blocks * p.tok_blocks);
@@ -272,6 +245,13 @@ static int launch_gemm(const GemmParams &p, cudaStream_t stream) {
   PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
   note_launches(1);
   return PARO_OK;
+}
+
+template <typename T>
+static int launch_gemm_nt(const GemmParams &p, cudaStream_t stream) {
+  if (p.NT == 128) return launch_gemm<T, 128>(p, stream);
+  if (p.NT == 64) return launch_gemm<T, 64>(p, stream);
+  return launch_gemm<T, 32>(p, stream);
 }
 
 int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
@@ -307,8 +287,8 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
   }
   p.rec_off = static_cast<long long>(L.rec_off);
   p.xr_part_stride = static_cast<long long>(m_pad) * L.K * 2;
-  if (s.dtype == PARO_BF16) return launch_gemm<__nv_bfloat16>(p, stream);
-  return launch_gemm<__half>(p, stream);
+  if (s.dtype == PARO_BF16) return launch_gemm_nt<__nv_bfloat16>(p, stream);
+  return launch_gemm_nt<__half>(p, stream);
 }
 
 }  // namespace paro

@@ -14,8 +14,8 @@
 //   weights  [t = 0..7][c = 0..3][row = 0..15] 16 bytes = 4 words; word j holds the 8 INT4 weights
 //            W[kb .. kb+7][n], n = 128*block + 16t + row, kb = 128*g + 32c + 8j, at bit positions
 //            0,16,4,20,8,24,12,28 -- so (w >> 4i) & 0x000F000F is the pair (kb+2i, kb+2i+1) sitting in
-//            the low mantissa bits of a bf16x2 / half2 word, i.e. the payload of one 32-bit TMEM column
-//            of the tcgen05 A operand (lane = output column n, TMEM column = k/2).
+//            the low mantissa bits of a bf16x2 / half2 word, i.e. one 32-bit register of an mma.sync / wgmma
+//            A fragment (row = output column n, channels kb+2i, kb+2i+1).
 //            One thread dequantises one COLUMN: 64 contiguous-in-k bytes per record, read as 4 x 16 B
 //            with the 16 rows of a chunk adjacent (conflict-free 128-bit shared loads).   (8192 bytes)
 //   scales   [128] T       s[g][n]                                                       (256 bytes)
@@ -45,7 +45,7 @@
 namespace paro {
 
 constexpr int kGroup = 128;
-constexpr int kBlockN = 128;               // output columns per block = TMEM lanes of one tcgen05.mma
+constexpr int kBlockN = 128;               // output columns per block = rows of the weight operand per round
 constexpr int kBlockWeightBytes = 8192;    // 128 columns x 128 channels of INT4
 constexpr int kBlockScaleOff = 8192;        // [qhalves][128] T, then [qhalves][128] uint8 zeros
 constexpr int kBlockBytes = 8192 + 256 + 128;      // group_size 128: one scale / zero set per record

@@ -65,7 +65,7 @@ __global__ void prepack_meta_kernel(Layout L, const int16_t *__restrict__ pairs,
 }
 
 // bit position of k-offset e (0..7) inside a word: consecutive k pairs land in the two 16-bit halves
-// so that (w >> 4i) & 0x000F000F is the bf16x2 / half2 payload of TMEM column i of the word
+// so that (w >> 4i) & 0x000F000F is the bf16x2 / half2 payload of the A-fragment register of channel pair i of the word
 __device__ __constant__ int kNibblePos[8] = {0, 16, 4, 20, 8, 24, 12, 28};
 
 // block index over all partitions -> partition

@@ -1,4 +1,4 @@
-// Standalone scaled pairwise (Givens) rotation for sm_100a -- the torch.ops.rotation.rotate
+// Standalone scaled pairwise (Givens) rotation for sm_90a -- the torch.ops.rotation.rotate
 // surface (/root/reference/paroquant/kernels/cuda/rotation.cu:10-43,62-135) and the
 // activation pre-pass of the large-M GEMM path.
 //
@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
 #pragma unroll
           for (int c = 0; c < 4; ++c) pr[c] = v[r][c];
           if (tiled_nt) {
-            // B-operand order of the tcgen05 GEMM (paro_gemm.cu): [token block][k16 step][k half][n/8][n%8][8 elems]
+            // B-operand order of the wgmma GEMM (paro_gemm.cu): [token block][k16 step][k half][n/8][n%8][8 elems]
             const int64_t m = row0 + r;
             const int64_t tb = m / tiled_nt;
             const int n = static_cast<int>(m - tb * tiled_nt), k = g * G + lane * 4;
@@ -212,7 +212,7 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
 }
 
 
-// ------------------------------------------------------------------ pre-pass of the tcgen05 kernels (paro_decode.cu from 5 rows, paro_gemm.cu)
+// ------------------------------------------------------------------ pre-pass of the tensor-core kernels (paro_decode.cu from 5 rows, paro_gemm.cu)
 // ONE launch for all partitions of a merged linear: warp = (partition, group, block of 8 rows); output in the B-operand order
 // of the consumer (tiles of nt tokens, rows >= M zero).  Same arithmetic as rotate_kernel; what differs is latency: the pair
 // indices and angles of all (<= 8 at a time) rotations are fetched up front, so the launch costs one global-load round trip
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const T *__restrict__
   T *o = out + part * out_part_elems;
   uint4 *rot = tile[warp];
   const int row0 = rb * RB;
-  // B-operand order of the tcgen05 kernels: [token block of nt][k16 step][k half][row / 8][row % 8][8 elements]
+  // B-operand order of the tensor-core kernels: [token block of nt][k16 step][k half][row / 8][row % 8][8 elements]
   auto tiled = [&](int m, int k) -> int64_t {
     const int tb = m / nt, n = m - tb * nt;
     return (static_cast<int64_t>(tb) * (K / 16) + (k >> 4)) * (static_cast<int64_t>(nt) * 16) + ((k >> 3) & 1) * (nt * 8) + (n >> 3) * 64 + (n & 7) * 8 +
@@ -532,7 +532,10 @@ static int launch_backward_T(const void *y, const void *gout, const void *x, con
   const int ctas_per_sm = resident < 1 ? 1 : resident > 6 ? 6 : resident;   // 6: the register limit
   // enough warps to fill the machine, no more splits than row blocks: every warp then walks ~row_blocks / splits blocks of its
   // group, computes the group's (cos, sin) once and pays its atomics once
-  int64_t splits = (148 * ctas_per_sm * 4 + groups - 1) / groups;
+  int dev = 0, sms = 0;
+  PARO_CUDA_OK(cudaGetDevice(&dev));
+  PARO_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int64_t splits = (static_cast<int64_t>(sms) * ctas_per_sm * 4 + groups - 1) / groups;
   if (splits > row_blocks) splits = row_blocks;
   if (splits < 1) splits = 1;
   const int64_t blocks = (splits * groups + 3) / 4;
@@ -567,7 +570,7 @@ int rotate_backward_launch(const void *y, const void *gout, const void *x, const
 }
 
 // Rotation pre-pass of the large-M path: the raw metadata of ONE partition, output in the B-operand tile
-// order of the tcgen05 GEMM, zero rows up to M_store (a multiple of tiled_nt).
+// order of the wgmma GEMM, zero rows up to M_store (a multiple of tiled_nt).
 int rotate_tiled_launch(const void *x, void *out, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
                         int scales_dtype, int64_t M, int64_t M_store, int tiled_nt, int K, int krot, int dtype, cudaStream_t stream) {
   if (dtype == PARO_F16)

@@ -6,15 +6,12 @@
 //
 // Formulation (operand-swapped, as the large-M kernel): D[n, m] += W[n, k] * x_rot[m, k]
 //   A = 128 output columns x 128 channels (one quantisation group) per ROUND, dequantised by CUDA cores straight
-//       into TENSOR MEMORY (tcgen05.st); thread = one output column = one TMEM lane.  kStmABufs = 7 A buffers are
-//       handed out round-robin (round rr -> buffer rr % 7) to the SETS = 5 dequant sets (round rr -> set rr % 5), so a
-//       set never waits for the tensor pipe to drain the buffer of its own previous round.
-//   B = x_rot of the CTA's K-slice, written once per step after the in-kernel rotation, UMMA K-major core-matrix order.
-//       For M <= 8 only 8 token rows are stored: the descriptor's 8-row-group stride is 0, so rows 8..15 of the
-//       N = 16 MMA alias rows 0..7 (their results are never read).
-//   D = fp32 [128 x 16] in TMEM, kStmDBufs = 4 accumulators.  All rounds of a SEGMENT (a run of one 128-column block's
-//       groups) accumulate into the same D whichever set produced A: the tensor core does the in-CTA part of the
-//       split-K reduction; a dedicated epilogue warp group reads D back (tcgen05.ld) off the dequant sets' critical path.
+//       into mma.sync A fragments (registers); warp = one 16-row tile of the block x one 64-channel half of every round.
+//   B = x_rot of the CTA's K-slice, written once per step after the in-kernel rotation, K-major core-matrix order, read
+//       as mma.sync B fragments.  For M <= 8 only 8 token rows are stored (one n8 tile).
+//   D = fp32 [16 x 16] per warp in registers over the rounds of a SEGMENT (a run of one 128-column block's groups); at
+//       the segment's end every warp writes its k half to one of kStmDBufs shared-memory accumulators and a dedicated
+//       epilogue warp group adds the two halves (fixed order) off the workers' critical path.
 //
 // Work split (no clusters; every SM works): the CTAs are dealt to `c` K-slices (whole groups, ragged), inside a slice
 // to the partitions of a merged linear (proportional to their 128-column blocks), and inside such a TEAM the rounds
@@ -25,14 +22,13 @@
 //
 // Chain: step i + 1 may take its x from step i.  The weight stream does not depend on activations, so the TMA
 // producer runs ahead across step boundaries (the ring holds the next step's first records while the current step
-// drains); TMEM allocation, barrier initialisation and the instruction cache are paid once.  The only serial part
+// drains); barrier initialisation and the instruction cache are paid once.  The only serial part
 // left between dependent steps is: last block fixed up -> step counter -> x load -> rotation -> first MMA.
 //   x ops:     NONE | SILU_MUL (x = T(silu(g)) * u of the [M, 2K] gate_up output) | RMSNORM (x = T(T(h * rstd) * w))
 //   epilogues: STORE | ADD_RESIDUAL (h = T(y + residual) -> residual_out, per-block sum of h^2 -> the next step's rstd)
 //
-// Roles: warps 0..4*SETS-1 dequant workers (TMEM lane quarter = warp % 4; they also run the rotation prologue);
-// 4 epilogue warps; 1 TMA producer warp (ONE 8576-byte record per round per cp.async.bulk); 1 MMA issuer warp (one
-// elected lane) that also owns the TMEM allocation.
+// Roles: warps 0..15 workers (tile = warp % 8, k half = warp / 8; they also run the rotation prologue); 4 epilogue
+// warps; 1 TMA producer warp (ONE 8576-byte record per round per cp.async.bulk).
 //
 // Numerics: x_rot as paro_rotate.cu; W = T((q - z) * T(s)) with ONE rounding (the operand Marlin / AWQ form); fp32
 // accumulation; one rounding to T.
@@ -49,15 +45,11 @@ namespace paro {
 
 constexpr int kStmMaxSteps = PARO_CHAIN_MAX_STEPS;
 constexpr int kStmMaxStages = 24;
-constexpr int kStmSets = 5;    // dequant sets of 4 warps (4 and 6 were measured: no better)
-constexpr int kStmABufs = 7;
-constexpr int kStmDBufs = 4;
-constexpr int kStmTmemCols = 512;
-constexpr uint32_t kStmDCol0 = 64 * kStmABufs;   // 448; D buffers take the last 64 columns
-constexpr int kStmN = 16;                        // MMA N (M_mma = 128 needs N % 16 == 0)
+constexpr int kStmSets = 4;    // worker warps = 4 x sets = 8 row tiles x 2 k halves
+constexpr int kStmDBufs = 2;   // segment accumulators handed to the epilogue group: [kStmDBufs][k half][M][128] fp32
 constexpr int kStmSmemLimit = 227 * 1024;
 // ring stage = one record: StreamParams::stage_bytes = the largest record of the chain's steps (8576, or 8960 with group_size 64)
-constexpr int kStmBarBytes = 16 * kStmMaxStages + 320;   // barriers (224 bytes after the ring's) + 16 rstd floats
+constexpr int kStmBarBytes = 16 * kStmMaxStages + 320;   // barriers (32 bytes after the ring's) + 16 rstd floats at +224
 constexpr int kStmMiscBytes = 4096;              // epilogue scratch: per warp, 64 segments x {block, global block, contributors, my slot | reducer}
 
 constexpr int kStmTraceSlots = 12;
@@ -101,7 +93,7 @@ struct StreamParams {
   int n_steps, M;
   int nstages, nrows_b;       // ring stages; B-operand rows stored per group (8 or 16)
   int rot_bytes, rot_warps;
-  int xb_off, rot_off, misc_off, bar_off;
+  int xb_off, rot_off, misc_off, dbuf_off, bar_off;
   int trace, inflight;        // inflight: bulk copies outstanding per SM
   int stage_bytes;            // ring stage stride
   uint32_t *sync;             // [0] epoch (tag of a launch = epoch + 1), [1] CTAs done
@@ -447,52 +439,34 @@ __device__ __forceinline__ void stm_prologue(const StepDesc &S, int M, int NR, R
 // ------------------------------------------------------------------ the kernel
 // MB: compile-time bound on the rows (M <= MB in {1, 4, 16}) -- sizes the epilogue's per-row registers
 template <typename T, int SETS, int MB>
-__global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __grid_constant__ StreamParams p) {
+__global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __grid_constant__ StreamParams p) {
+  static_assert(SETS == 4, "the workers are 8 row tiles x 2 k halves");
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int kWorkers = 4 * SETS;
-  constexpr int kEpiWarp0 = kWorkers, kProdWarp = kWorkers + 4, kMmaWarp = kWorkers + 5;
+  constexpr int kEpiWarp0 = kWorkers, kProdWarp = kWorkers + 4;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int cta = blockIdx.x;
   const long long t_entry = clock64();
   const int NS = p.nstages, NR = p.nrows_b, M = p.M, nsteps = p.n_steps;
   const uint32_t smem0 = smem_u32(smem);
-  const uint32_t xb = smem0 + p.xb_off, bars = smem0 + p.bar_off;
+  const uint32_t xb = smem0 + p.xb_off, bars = smem0 + p.bar_off, dbuf = smem0 + p.dbuf_off;
   const uint32_t bar_wfull = bars, bar_wempty = bars + 8 * kStmMaxStages;
-  const uint32_t bar_afull = bars + 16 * kStmMaxStages, bar_afree = bar_afull + 64;
-  const uint32_t bar_dfull = bar_afull + 128, bar_dfree = bar_afull + 160;
-  const uint32_t bar_xb = bar_afull + 192, bar_stepdone = bar_afull + 200, tmem_slot = bar_afull + 208;
+  const uint32_t bar_dfull = bars + 16 * kStmMaxStages, bar_dfree = bar_dfull + 16;
+  const uint32_t dbuf_bytes = 2u * M * 512;   // one segment accumulator: [k half][M][128] fp32
 
   if (warp == kProdWarp) {
+    // every worker warp consumes every ring stage and contributes to every segment accumulator
     if (lane < NS) {
       mbar_init(bar_wfull + 8 * lane, 1);
-      mbar_init(bar_wempty + 8 * lane, 4);
-    }
-    // Every barrier has ONE waiting party that consumes its phases in order (a parity wait issued a phase early passes
-    // on the stale phase).  Ring stages are always consumed by the same set (the stage count is a multiple of SETS).
-    // A buffers are shared by the sets, but the set that waits for the drain of round rr - 7 has already waited for
-    // round rr - 5 - 7, and drains complete in issue order, so it is never two phases ahead (needs kStmABufs >= SETS).
-    if (lane < kStmABufs) {
-      mbar_init(bar_afull + 8 * lane, 4);
-      mbar_init(bar_afree + 8 * lane, 1);
+      mbar_init(bar_wempty + 8 * lane, kWorkers);
     }
     if (lane < kStmDBufs) {
-      mbar_init(bar_dfull + 8 * lane, 1);
+      mbar_init(bar_dfull + 8 * lane, kWorkers);
       mbar_init(bar_dfree + 8 * lane, 4);
-    }
-    if (lane == 0) {
-      mbar_init(bar_xb, kWorkers);
-      mbar_init(bar_stepdone, 1);
     }
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kStmTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = lds32(tmem_slot);
   pdl_launch_dependents();   // the next kernel in the stream may start its own prologue as soon as SMs free up
 
   if (warp == kProdWarp) {
@@ -532,61 +506,14 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __
         }
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ================= MMA issuer.  The whole warp runs the loop (waits included) and ONE elected lane issues (under a
-    // plain `lane == 0` branch ptxas wraps every tcgen05.mma in a divergence loop, tools/mma_probe.cu).
-    const uint32_t idesc = instr_desc<T>(kStmN);
-    const uint64_t desc_hi = smem_desc_kmajor(0, NR * 16, NR == 16 ? 128 : 0);   // everything but the start address
-    int a = 0, ause = 0, d = 0, duse = 0;
-#pragma unroll 1
-    for (int i = 0; i < nsteps; ++i) {
-      const StepDesc &S = p.steps[i];
-      const StepGeom g = step_geom(S, cta);
-      mbar_wait(bar_xb, i & 1);   // B operand rows written (generic proxy) and fenced by the workers
-      tc_fence_after();
-      if (g.active) {
-        const SegWalk sw = seg_walk(g);
-#pragma unroll 1
-        for (int k = 0; k < sw.nseg; ++k) {
-          int ra, rb;
-          seg_range(sw, k, ra, rb);
-          int gi = ra - static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng)) * g.ng;
-          if (duse > 0) mbar_wait(bar_dfree + 8 * d, (duse - 1) & 1);   // accumulator read back by the epilogue group
-          const uint32_t td = tmem + kStmDCol0 + d * kStmN;
-#pragma unroll 1
-          for (int r = ra; r < rb; ++r, ++gi) {
-            mbar_wait(bar_afull + 8 * a, ause & 1);
-            tc_fence_after();
-            const uint32_t ta = tmem + a * 64;
-            const uint64_t bdesc0 = desc_hi | static_cast<uint64_t>(((xb + gi * (NR * 256)) >> 4) & 0x3FFF);
-            if (elect_one()) {
-#pragma unroll
-              for (int s = 0; s < 8; ++s) tc_mma_ts(td, ta + 8 * s, bdesc0 + s * ((NR * 32) >> 4), idesc, (r == ra && s == 0) ? 0u : 1u);
-              tc_commit(bar_afree + 8 * a);
-              if (r == rb - 1) tc_commit(bar_dfull + 8 * d);
-            }
-            __syncwarp();
-            if (++a == kStmABufs) { a = 0; ++ause; }
-          }
-          if (++d == kStmDBufs) { d = 0; ++duse; }
-        }
-        if (elect_one()) tc_commit(bar_stepdone);   // arrives when every MMA of this step has read its operands
-        __syncwarp();
-        STM_TRACE(i, 10);
-      } else {
-        if (lane == 0) mbar_arrive(bar_stepdone);
-        __syncwarp();
-      }
-    }
   } else if (warp >= kEpiWarp0) {
-    // ================= epilogue group (4 warps, TMEM lane quarter = warp % 4; each warp works alone on its 32 columns):
+    // ================= epilogue group (4 warps, thread = one of the block's 128 columns; each warp works alone on its 32 columns):
     // D -> {partial, tag} slot; the block's REDUCER (in K slice `block mod c`, the contributor that holds the block's last round)
     // looks at the other contributors' slots, adds them in fixed order, finishes the block and publishes it for the next step,
     // again as {value, tag} words.  No fences, no counters: every 8-byte word carries the launch's tag, a reader retries
     // until the tag matches.
     const int q = warp & 3;
     const int L128 = 32 * q + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(32 * q) << 16;
     int d = 0, duse = 0;
     uint32_t tag = 0;
     bool have_tag = false;
@@ -742,19 +669,18 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __
           }
         }
         if (k == sw.nseg) break;
-        tc_fence_after();
         if (warp == kEpiWarp0) STM_TRACE(i, 8);
         if (!have_tag) {   // the workers are past griddepcontrol.wait: the previous launch has bumped the epoch
           tag = ld_relaxed_u32(p.sync) + 1u;
           have_tag = true;
         }
-        uint32_t v[16];
-        if constexpr (MB == 1) tc_ld1(tmem + lane_base + kStmDCol0 + d * kStmN, v[0]);
-        else if constexpr (MB == 4) tc_ld4(tmem + lane_base + kStmDCol0 + d * kStmN, v);
-        else if (M <= 8) tc_ld8(tmem + lane_base + kStmDCol0 + d * kStmN, v);
-        else tc_ld16(tmem + lane_base + kStmDCol0 + d * kStmN, v);
-        tc_wait_ld();
-        tc_fence_before();
+        uint32_t v[MB] = {};
+        {
+          const uint32_t db = dbuf + d * dbuf_bytes + L128 * 4;   // the two k halves, added in a fixed order
+#pragma unroll
+          for (int m = 0; m < MB; ++m)
+            if (m < M) v[m] = __float_as_uint(lds_f32(db + m * 512) + lds_f32(db + (M + m) * 512));
+        }
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_dfree + 8 * d);
         if (++d == kStmDBufs) { d = 0; ++duse; }
@@ -779,20 +705,14 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __
       if (warp == kEpiWarp0) STM_TRACE(i, 6);
     }
   } else {
-    // ================= dequant workers
-    const int wi = warp, e = wi >> 2, q = warp & 3;
-    const int L128 = 32 * q + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(32 * q) << 16;
-    const uint32_t col_off = (L128 >> 4) * 1024 + (L128 & 15) * 16;   // my 16-byte slots inside a record's weights
+    // ================= workers: warp = (16-row tile of the block, k half of every record); each takes every round
+    const int wi = warp, tile = warp & 7, kh = warp >> 3;
     const uint32_t rot = smem0 + p.rot_off + wi * p.rot_bytes;
     const int nq = M > 4 ? (M + 3) >> 2 : 1;   // rotation tasks: row blocks of 4 for M > 4
-    uint32_t rr_base = 0;                      // global round index (over all steps) of this step's first round
     uint32_t tag = 0;
     const uint32_t rstd_smem = bars + 16 * kStmMaxStages + 224;   // 16 floats behind the barriers
-    // my next round: rr; ring stage / parity, A buffer / use derived incrementally
-    uint32_t rr = e;
-    int st = e, par = 0, a = e, ause = 0;
-    while (st >= NS) { st -= NS; par ^= 1; }   // (NS >= SETS always)
+    const int g8 = lane >> 2, t4 = lane & 3;
+    int st = 0, par = 0, d = 0, duse = 0;
 #pragma unroll 1
     for (int i = 0; i < nsteps; ++i) {
       const StepDesc &S = p.steps[i];
@@ -811,10 +731,10 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __
         if (wi == 0) STM_TRACE(0, 0);
         pdl_wait();   // x may have been written by the previous kernel in the stream
         tag = ld_relaxed_u32(p.sync) + 1u;   // ... which has also bumped the epoch
+      } else {
+        named_bar_sync(2, 32 * kWorkers);   // every worker is done with the previous step's B operand
       }
       if (wi == 0) STM_TRACE(i, 1);
-      // the previous step's MMAs no longer read the B operand (every worker warp waits, so each consumes the phases in order)
-      if (i > 0) mbar_wait(bar_stepdone, (i - 1) & 1);
       if (mine) {
         if (S.x_op == PARO_XOP_RMSNORM) {
           const int nrot = ntasks < p.rot_warps ? ntasks : p.rot_warps;   // the warps that rotate in this step (warp 0 is one)
@@ -830,74 +750,51 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 6), 1) stream_kernel(const __
         } else {
           stm_prologue<T, 4>(S, M, NR, rm, g, ntasks, nq, wi, p.rot_warps, lane, rot, xb, tag, rstd_smem);
         }
-        fence_proxy_async_smem();  // B rows were written through the generic proxy, tcgen05.mma reads them through the async proxy
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_xb);
+      named_bar_sync(2, 32 * kWorkers);   // B operand of this step complete
       if (wi == 0) STM_TRACE(i, 3);
+      if (!g.active) continue;
 
-      const uint32_t nr = static_cast<uint32_t>(g.r1 - g.r0);
-      const uint32_t rr_end = rr_base + nr;
       const bool q2 = S.q2 != 0;
       const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
+      const SegWalk sw = seg_walk(g);
       bool first = true;
 #pragma unroll 1
-      for (; rr < rr_end; rr += SETS) {
-        mbar_wait(bar_wfull + 8 * st, par);
-        if (first) { if (wi == 0) STM_TRACE(i, 4); first = false; }
-        const uint32_t rec = smem0 + st * p.stage_bytes;
-        RowDequant<T> dq;
-        dq.prep(lds16(rec + kBlockScaleOff + 2 * L128), lds8(rec + zero_off + L128));
-        uint32_t s_hi = 0, z_hi = 0;   // group_size 64: channels 64..127 of the record have their own scale / zero
-        if (q2) { s_hi = lds16(rec + kBlockScaleOff + 256 + 2 * L128); z_hi = lds8(rec + zero_off + 128 + L128); }
-        const uint32_t wbase = rec + col_off;
-        const uint32_t ta = tmem + lane_base + a * 64;
-        // the first chunk is dequantised before the wait for the A buffer (it only needs registers)
-        uint4 w4 = lds128(wbase);
-        uint32_t regs[16];
-        dq.word(w4.x, regs + 0);
-        dq.word(w4.y, regs + 4);
-        dq.word(w4.z, regs + 8);
-        dq.word(w4.w, regs + 12);
-        if (ause > 0) mbar_wait(bar_afree + 8 * a, (ause - 1) & 1);  // the MMAs of round rr - 7 have drained this A buffer
-        tc_fence_after();
-        tc_st16(ta, regs);
+      for (int k = 0; k < sw.nseg; ++k) {
+        int ra, rb;
+        seg_range(sw, k, ra, rb);
+        int gi = ra - static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng)) * g.ng;
+        float acc[2][4] = {};
+#pragma unroll 1
+        for (int r = ra; r < rb; ++r, ++gi) {
+          mbar_wait(bar_wfull + 8 * st, par);
+          if (first) { if (wi == 0) STM_TRACE(i, 4); first = false; }
+          const uint32_t rec = smem0 + st * p.stage_bytes, xbg = xb + gi * (NR * 256);
+          if (M > 8) mma_round<T, 2>(rec, q2, zero_off, xbg, NR, tile, kh, lane, acc);
+          else mma_round<T, 1>(rec, q2, zero_off, xbg, NR, tile, kh, lane, acc);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_wempty + 8 * st);
+          if (++st == NS) { st = 0; par ^= 1; }
+        }
+        // ---- segment done: my k half of the accumulator to the epilogue group
+        if (duse > 0) mbar_wait(bar_dfree + 8 * d, (duse - 1) & 1);
+        const uint32_t db = dbuf + d * dbuf_bytes + (kh * M) * 512;
 #pragma unroll
-        for (int c = 1; c < 4; ++c) {
-          w4 = lds128(wbase + c * 256);
-          uint32_t r2[16];
-          if (c == 2 && q2) dq.prep(s_hi, z_hi);
-          dq.word(w4.x, r2 + 0);
-          dq.word(w4.y, r2 + 4);
-          dq.word(w4.z, r2 + 8);
-          dq.word(w4.w, r2 + 12);
-          tc_st16(ta + 16 * c, r2);
+        for (int e = 0; e < 8; ++e) {
+          const int col = 16 * tile + g8 + 8 * ((e >> 1) & 1), m = 8 * (e >> 2) + 2 * t4 + (e & 1);
+          if (m < M) sts_f32(db + m * 512 + col * 4, acc[e >> 2][e & 3]);
         }
-        tc_wait_st();
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(bar_afull + 8 * a);
-          mbar_arrive(bar_wempty + 8 * st);
-        }
-        st += SETS;
-        if (st >= NS) { st -= NS; par ^= 1; }
-        a += SETS;
-        if (a >= kStmABufs) { a -= kStmABufs; ++ause; }
+        if (lane == 0) mbar_arrive(bar_dfull + 8 * d);
+        if (++d == kStmDBufs) { d = 0; ++duse; }
       }
-      rr_base = rr_end;
       if (wi == 0) STM_TRACE(i, 5);
     }
   }
 
   // ================= common tail
   __syncwarp();
-  tc_fence_before();
   __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kStmTmemCols) : "memory");
-  }
   if (threadIdx.x == 0) {
     // the last CTA to get here bumps the epoch: every tag of this launch becomes stale, the next launch on this workspace
     // (which reads the epoch after griddepcontrol.wait, i.e. after this grid has completed) uses a fresh one
@@ -1001,7 +898,8 @@ static bool stm_choose_plan(const Layout &L, int M, int sets, int ctas, int forc
     if (!stm_deal_members(L, pl.T, pl.part_cta_begin)) continue;
     pl.ng_max = (L.groups + c - 1) / c;
     const int xb_bytes = pl.ng_max * NR * 256;
-    const int nst_room = (kStmSmemLimit - xb_bytes - 4 * sets * kGroup * 2 * stm_rot_rows(M) - kStmBarBytes - kStmMiscBytes - 256) / kBlockBytesMax / sets * sets;
+    const int nst_room = (kStmSmemLimit - xb_bytes - 4 * sets * kGroup * 2 * stm_rot_rows(M) - kStmBarBytes - kStmMiscBytes - kStmDBufs * M * 1024 - 256) /
+                         kBlockBytesMax / sets * sets;
     if (nst_room < sets) continue;
     pl.max_rounds = 0;
     pl.max_slots = 1;
@@ -1098,7 +996,7 @@ bool stream_supported(const Layout &L, int64_t M) { return M >= 1 && M <= 16 && 
 size_t stream_sync_bytes(const Layout &) { return kStmSyncBytes; }
 size_t stream_workspace_bytes(const Layout &L, int64_t max_m) {
   const int sms = stm_device_sms();
-  const int ctas = sms > 0 ? sms : 148;
+  const int ctas = sms > 0 ? sms : 132;
   size_t need = kStmSyncBytes;
   const int top = max_m < 16 ? static_cast<int>(max_m) : 16;
   for (int M = 1; M <= top; ++M) {
@@ -1122,7 +1020,7 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
   const int xb_bytes = max_ng * p.nrows_b * 256;
   for (;;) {
     const int rot_total = (rw * p.rot_bytes + 127) / 128 * 128;
-    const int fixed = xb_bytes + rot_total + kStmMiscBytes + kStmBarBytes + 128;
+    const int fixed = xb_bytes + rot_total + kStmMiscBytes + kStmDBufs * M * 1024 + kStmBarBytes + 128;
     int nst = (kStmSmemLimit - fixed) / p.stage_bytes;
     if (nst > kStmMaxStages) nst = kStmMaxStages;
     if (kn.stages >= SETS && kn.stages < nst) nst = kn.stages;
@@ -1134,7 +1032,8 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
       p.xb_off = (nst * p.stage_bytes + 127) / 128 * 128;
       p.rot_off = p.xb_off + xb_bytes;
       p.misc_off = p.rot_off + rot_total;
-      p.bar_off = p.misc_off + kStmMiscBytes;
+      p.dbuf_off = p.misc_off + kStmMiscBytes;
+      p.bar_off = p.dbuf_off + kStmDBufs * M * 1024;
       break;
     }
     if (rw <= 2) { set_error("decode: no launch configuration fits (M=%d, %d groups per CTA)", M, max_ng); return PARO_EUNSUPPORTED; }
@@ -1156,7 +1055,7 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(32 * (4 * SETS + 6));
+  cfg.blockDim = dim3(32 * (4 * SETS + 5));
   cfg.dynamicSmemBytes = smem_total;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
@@ -1175,7 +1074,7 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
 
 size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) {
   const int sms = stm_device_sms();
-  const int ctas = sms > 0 ? sms : 148;
+  const int ctas = sms > 0 ? sms : 132;
   size_t off = kStmSyncBytes;
   for (int i = 0; i < n; ++i) {
     StepPlan pl;

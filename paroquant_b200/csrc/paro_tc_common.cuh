@@ -1,5 +1,5 @@
 // Device helpers shared by the tensor-core kernels (paro_decode.cu, paro_gemm.cu):
-// tcgen05 / TMEM wrappers, UMMA descriptors, cluster + DSMEM primitives, the INT4 -> T row dequant
+// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T row dequant
 // and the in-warp pairwise rotation (rounding points of /root/reference/paroquant/kernels/cuda/rotation.cuh:91-173).
 #pragma once
 #include "paro_common.cuh"
@@ -13,66 +13,96 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   return t;
 }
 
-// ------------------------------------------------------------------ tcgen05 wrappers
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem_d] (+)= A[tmem_a] * B[smem desc]; A: 128 lanes x 8 columns (16 x 16-bit k), kind::f16
-__device__ __forceinline__ void tc_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld2(uint32_t taddr, uint32_t &a, uint32_t &b) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(a), "=r"(b) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld1(uint32_t taddr, uint32_t &a) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(a) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld4(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// ------------------------------------------------------------------ tensor-core operands
+// Both fused small-M kernels (paro_decode.cu, paro_stream.cu) and the large-M GEMM (paro_gemm.cu) work operand-swapped:
+// D[n, m] += W[n, k] * x_rot[m, k], the dequantised weights are the register A operand, x_rot the shared-memory B operand.
+// A warp owns a 16-row tile of the 128-column block; its A fragment (mma.m16n8k16 and one warp's slice of a wgmma m64) holds
+// rows g = lane / 4 and g + 8, channels 2t, 2t + 1 and 2t + 8, 2t + 9 of each k16 step (t = lane % 4).
+
+// D (fp32, 16 x 8) += A (16 x 16) * B (16 x 8)
+template <typename T>
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t *a, uint32_t b0, uint32_t b1) {
+  if constexpr (Traits<T>::code == PARO_BF16)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// K-major, no swizzle: 8-row x 16-byte core matrices; `lbo` = byte distance between the two k-halves
-// of a k16 step, `sbo` = byte distance between 8-row groups (cute::UMMA::SmemDescriptor, version 1)
+// K-major, no swizzle: 8-row x 16-byte core matrices; `lbo` = byte distance between the two k-halves of a k16 step,
+// `sbo` = byte distance between 8-row groups (wgmma matrix descriptor, swizzle mode 0)
 __device__ __forceinline__ uint64_t smem_desc_kmajor(uint32_t addr, uint32_t lbo, uint32_t sbo) {
   return static_cast<uint64_t>((addr >> 4) & 0x3FFF) | (static_cast<uint64_t>((lbo >> 4) & 0x3FFF) << 16) |
-         (static_cast<uint64_t>((sbo >> 4) & 0x3FFF) << 32) | (1ull << 46);
+         (static_cast<uint64_t>((sbo >> 4) & 0x3FFF) << 32);
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (bit 4), a/b format (bits 7, 10: 0 = F16, 1 = BF16), K-major A and B,
-// N >> 3 at bit 17, M >> 4 at bit 24
-template <typename T> __device__ __forceinline__ uint32_t instr_desc(int n) {
-  const uint32_t fmt = Traits<T>::code == PARO_BF16 ? 1u : 0u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (8u << 24);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R> __device__ __forceinline__ void fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// D (fp32, 64 x N, the warpgroup's registers) += A (64 x 16, registers) * B (16 x N, shared memory descriptor, K-major)
+template <typename T, int N> struct Wgmma;
+template <> struct Wgmma<__nv_bfloat16, 32> {
+  __device__ static __forceinline__ void mma(float (&d)[16], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
+template <> struct Wgmma<__half, 32> {
+  __device__ static __forceinline__ void mma(float (&d)[16], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
+template <> struct Wgmma<__nv_bfloat16, 64> {
+  __device__ static __forceinline__ void mma(float (&d)[32], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
+template <> struct Wgmma<__half, 64> {
+  __device__ static __forceinline__ void mma(float (&d)[32], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
+template <> struct Wgmma<__nv_bfloat16, 128> {
+  __device__ static __forceinline__ void mma(float (&d)[64], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
+template <> struct Wgmma<__half, 128> {
+  __device__ static __forceinline__ void mma(float (&d)[64], const uint32_t *a, uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+  }
+};
 
 // one lane of a converged warp (CUTLASS' elect_one_sync): ptxas treats the guarded region as single-threaded
 __device__ __forceinline__ bool elect_one() {
@@ -137,32 +167,59 @@ template <> struct RowDequant<__nv_bfloat16> {
     const __nv_bfloat162 d = __hsub2(unpack2<__nv_bfloat16>(and_or(w, 0x000F000Fu, 0x43004300u)), unpack2<__nv_bfloat16>(z2));
     return pack2<__nv_bfloat16>(__hmul2(d, unpack2<__nv_bfloat16>(s2)));
   }
-  __device__ __forceinline__ void word(uint32_t w, uint32_t *r) const {
-    r[0] = one(w);
-    r[1] = one(w >> 4);
-    r[2] = one(w >> 8);
-    r[3] = one(w >> 12);
-  }
+  // pair t (channels 2t, 2t + 1) of a record word
+  __device__ __forceinline__ uint32_t pair(uint32_t w, int t) const { return one(w >> (4 * t)); }
 };
 
 template <> struct RowDequant<__half> {
-  uint32_t s2, z_lo, z_hi16;
+  uint32_t s2, z_lo;
   __device__ __forceinline__ void prep(uint32_t s_bits, uint32_t z) {
     s2 = s_bits * 0x00010001u;
-    z_lo = (0x6400u | z) * 0x00010001u;           // {1024 + z}
-    z_hi16 = (0xD400u | (z << 4)) * 0x00010001u;  // {-(64 + z)}
+    z_lo = (0x6400u | z) * 0x00010001u;   // {1024 + z}
   }
-  __device__ __forceinline__ void word(uint32_t w, uint32_t *r) const {
-    const uint32_t w8 = w >> 8;
-    const __half2 sixteenth = unpack2<__half>(0x2C002C00u), s = unpack2<__half>(s2);
-    // low nibble: 0x6400 | q = 1024 + q.  High nibble in place: 0x6400 | (q << 4) = 1024 + 16 q,
-    // and fma(1024 + 16 q, 1/16, -(64 + z)) = q - z exactly.
-    r[0] = pack2<__half>(__hmul2(__hsub2(unpack2<__half>(and_or(w, 0x000F000Fu, 0x64006400u)), unpack2<__half>(z_lo)), s));
-    r[1] = pack2<__half>(__hmul2(__hfma2(unpack2<__half>(and_or(w, 0x00F000F0u, 0x64006400u)), sixteenth, unpack2<__half>(z_hi16)), s));
-    r[2] = pack2<__half>(__hmul2(__hsub2(unpack2<__half>(and_or(w8, 0x000F000Fu, 0x64006400u)), unpack2<__half>(z_lo)), s));
-    r[3] = pack2<__half>(__hmul2(__hfma2(unpack2<__half>(and_or(w8, 0x00F000F0u, 0x64006400u)), sixteenth, unpack2<__half>(z_hi16)), s));
+  // 0x6400 | q = 1024 + q; (1024 + q) - (1024 + z) = q - z exactly, one rounding in the multiply
+  __device__ __forceinline__ uint32_t pair(uint32_t w, int t) const {
+    return pack2<__half>(__hmul2(__hsub2(unpack2<__half>(and_or(w >> (4 * t), 0x000F000Fu, 0x64006400u)), unpack2<__half>(z_lo)), unpack2<__half>(s2)));
   }
 };
+
+// A fragments of k16 steps 2c and 2c + 1 (channels 32c .. 32c + 31 of a record) for rows r and r + 8 of a 16-row tile
+// (r = 16 * tile + lane / 4): one 128-bit load per row -- the four lanes of a row read the same 16 bytes (paro_layout.h:
+// word j of a chunk holds channels 8j .. 8j + 7), each keeps its pair t = lane % 4 of every word.
+template <typename T>
+__device__ __forceinline__ void frag_a2(uint32_t rec, int r, int c, int t, const RowDequant<T> &d0, const RowDequant<T> &d1, uint32_t (&a)[8]) {
+  const uint32_t base = rec + (r >> 4) * 1024 + c * 256 + (r & 15) * 16;
+  const uint4 w0 = lds128(base), w1 = lds128(base + 128);
+  a[0] = d0.pair(w0.x, t); a[1] = d1.pair(w1.x, t); a[2] = d0.pair(w0.y, t); a[3] = d1.pair(w1.y, t);
+  a[4] = d0.pair(w0.z, t); a[5] = d1.pair(w1.z, t); a[6] = d0.pair(w0.w, t); a[7] = d1.pair(w1.w, t);
+}
+
+// One record (128 columns x 128 channels) of a small-M worker warp: its 16-row tile, k16 steps 4 kh .. 4 kh + 3, NTT token
+// tiles of 8.  B (x_rot of the record's group) is K-major core matrices: [k16 step][k half][row / 8][row % 8][8 elements],
+// NR rows per step (8 or 16).  group_size 64: channels 64..127 (kh = 1) have the record's second scale / zero set.
+template <typename T, int NTT>
+__device__ __forceinline__ void mma_round(uint32_t rec, bool q2, uint32_t zero_off, uint32_t xbg, int NR, int tile, int kh, int lane, float (&acc)[2][4]) {
+  const int g = lane >> 2, t = lane & 3, r = 16 * tile + g;
+  const uint32_t so = (q2 && kh) ? 256 : 0, zo = (q2 && kh) ? 128 : 0;
+  RowDequant<T> d0, d1;
+  d0.prep(lds16(rec + kBlockScaleOff + so + 2 * r), lds8(rec + zero_off + zo + r));
+  d1.prep(lds16(rec + kBlockScaleOff + so + 2 * (r + 8)), lds8(rec + zero_off + zo + r + 8));
+#pragma unroll
+  for (int cc = 0; cc < 2; ++cc) {
+    const int c = 2 * kh + cc;
+    uint32_t a[8];
+    frag_a2<T>(rec, r, c, t, d0, d1, a);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t bs = xbg + (2 * c + h) * (NR * 32) + t * 4;
+#pragma unroll
+      for (int nt = 0; nt < NTT; ++nt) {
+        const uint32_t ba = bs + nt * 128 + g * 16;
+        mma16816<T>(acc[nt], a + 4 * h, lds32(ba), lds32(ba + NR * 16));
+      }
+    }
+  }
+}
 
 // ------------------------------------------------------------------ in-warp rotation of one group
 // Tile `rot` = this warp's [128 channels][ROWS] elements of T, channel-major.  Lane owns pairs

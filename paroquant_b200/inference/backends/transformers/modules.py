@@ -4,7 +4,7 @@ Mirror of /root/reference/paroquant/inference/backends/transformers/modules.py:1
 buffers whose names are the checkpoint keys (`theta`, `pairs`, `channel_scales`, `qweight`,
 `qzeros`, `scales`, `bias`), so `load_state_dict` / `from_pretrained` fill them directly.  The
 reference's forward is rotate -> AutoAWQ GEMM (two kernels, fp16 only); here the first forward
-prepacks the buffers once and every forward is ONE fused sm_100a launch, fp16 or bf16.
+prepacks the buffers once and every forward is ONE fused sm_90a launch, fp16 or bf16.
 """
 from __future__ import annotations
 

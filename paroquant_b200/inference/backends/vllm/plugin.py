@@ -1,4 +1,4 @@
-"""vLLM quantisation plugin: `ParoQuantConfig` / `ParoQuantLinearMethod` on sm_100a.
+"""vLLM quantisation plugin: `ParoQuantConfig` / `ParoQuantLinearMethod` on sm_90a.
 
 Drop-in for /root/reference/paroquant/inference/backends/vllm/plugin.py (same registration name
 "paroquant", same parameter names / shapes / loaders, same TP input-dim sharding of the rotation
@@ -10,7 +10,7 @@ parameters), with a different engine underneath:
   AWQ -> Marlin repack per partition          one prepack into the streaming layout of csrc/
   apply(): n rotate + n Marlin + cat (+bias)  apply(): ONE fused launch for all partitions
   theta / scales cast to x.dtype per call     cast once at prepack
-  min capability 75                           100 (sm_100a only, no fallback path)
+  min capability 75                            90 (sm_90a only, no fallback path)
 """
 from __future__ import annotations
 
@@ -91,7 +91,7 @@ class ParoQuantConfig(QuantizationConfig):
 
     @classmethod
     def get_min_capability(cls) -> int:
-        return 100
+        return 90
 
     @classmethod
     def get_config_filenames(cls) -> list[str]:

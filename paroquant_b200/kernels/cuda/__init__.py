@@ -1,4 +1,4 @@
-"""`torch.ops.rotation.rotate` on sm_100a, plus the autograd wrapper.
+"""`torch.ops.rotation.rotate` on sm_90a, plus the autograd wrapper.
 
 Same operator surface as the reference's JIT-built extension
 (/root/reference/paroquant/kernels/cuda/__init__.py:52-65, rotation.cu:128-135): importing this

@@ -2,7 +2,7 @@
 
 Surface of /root/reference/paroquant/kernels/cuda/autograd.py:6-65 (`RotateTensorFunc`,
 `scaled_pairwise_rotation`) used by the offline optimiser and the checkpoint converter.
-Forward is the sm_100a kernel.  Backward is ONE launch (`paro_rotate_backward`,
+Forward is the sm_90a kernel.  Backward is ONE launch (`paro_rotate_backward`,
 csrc/paro_rotate.cu) where the reference walks the rotations in Python (per rotation two rotate
 launches, five gathers and a reduction).  It uses the identities
 

@@ -12,7 +12,7 @@ SMEM_LIMIT = 227 * 1024
 REC = {128: 8576, 64: 8960}   # record = ring stage: group_size 64 carries two scale / zero sets (paro_layout.h)
 
 
-def plan(K, parts, M, sets=5, sms=148, resident=(148, 74, 33, 16), group=128):
+def plan(K, parts, M, sets=5, sms=132, resident=(132, 66, 32, 16), group=128):
     shape = _cabi.make_shape(K, parts, group, 8, torch.bfloat16)
     out = (ctypes.c_int32 * 20)()
     res = (ctypes.c_int32 * 4)(*resident)
@@ -39,7 +39,7 @@ def test_plan_covers_the_layer_once_and_fits(K, parts, M, sets, group):
     c, groups = p["c"], K // 128
     blocks = [(n + 127) // 128 for n in parts]
     assert c in (1, 2, 4, 8) and c <= groups
-    assert p["grid"] == p["ranges"] * c and p["ranges"] <= (148, 74, 33, 16)[c.bit_length() - 1]
+    assert p["grid"] == p["ranges"] * c and p["ranges"] <= (132, 66, 32, 16)[c.bit_length() - 1]
     assert p["ranges"] >= len(parts) and prb[0] == 0 and prb[len(parts)] == p["ranges"]
     # ---- the kernel's index arithmetic (decode_kernel prologue), CTA by CTA
     seen = {}
@@ -79,7 +79,7 @@ def test_plan_uses_the_machine_for_the_llama_shapes():
     for K, parts, slack in ((4096, [14336, 14336], 1.2), (14336, [4096], 1.2), (4096, [4096], 1.2), (4096, [4096, 1024, 1024], 1.6)):
         p, _ = plan(K, parts, 1)
         units = sum((n + 127) // 128 for n in parts) * (K // 128)
-        assert p["nj_max"] * p["ng_max"] <= slack * units / 148 + 1, (K, parts, p)
+        assert p["nj_max"] * p["ng_max"] <= slack * units / 132 + 1, (K, parts, p)
         assert p["grid"] >= 96
     # large M: the DSMEM receive buffer must not crowd the weight ring down to one stage per set
     for K, parts in ((4096, [14336, 14336]), (4096, [4096]), (14336, [4096])):
@@ -88,9 +88,9 @@ def test_plan_uses_the_machine_for_the_llama_shapes():
 
 
 def test_plan_without_clusters_and_errors():
-    p, _ = plan(4096, [4096], 1, resident=(148, 0, 0, 0))
+    p, _ = plan(4096, [4096], 1, resident=(132, 0, 0, 0))
     assert p["c"] == 1 and p["grid"] == 32 and p["ng_max"] == 32          # one CTA per block, whole K
     with pytest.raises(RuntimeError, match="no launch configuration fits"):
-        plan(14336, [4096], 1, resident=(148, 0, 0, 0))                  # 112 groups of B operand do not fit one CTA
+        plan(14336, [4096], 1, resident=(132, 0, 0, 0))                  # 112 groups of B operand do not fit one CTA
     with pytest.raises(RuntimeError, match="bad M"):
         plan(4096, [4096], 17)

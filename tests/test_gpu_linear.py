@@ -5,7 +5,7 @@
   * fused linear vs the oracle on the same seeded inputs: normwise relative error <= 1e-3 in the
     activation dtype (BASELINE.json's tolerance); in practice ~1e-4 (MUFU flips in the rotation
     + fp32 accumulation order);
-  * vs fixtures of the unmodified reference pipeline (its rotate + vLLM Marlin) captured on a B200;
+  * vs fixtures of the unmodified reference pipeline (its rotate + vLLM Marlin) captured on an H100;
   * size-independent properties at BASELINE sizes.
 """
 import numpy as np
@@ -199,7 +199,7 @@ def test_vs_reference_pipeline_fixture(PK, path):
                                        (4096, [4096], 256), (4096, [4096, 1024, 1024], 300), (11008, [512], 33), (14336, [256], 257),
                                        (1152, [128], 40), (256, [272, 16], 33)])
 def test_large_m_gemm_vs_rotate_and_dense(PK, dt, K, parts, M):
-    """M > 16: rotation pre-pass + tcgen05 GEMM against fp64 matmul on the kernel's own dequantised operand and the
+    """M > 16: rotation pre-pass + wgmma GEMM against fp64 matmul on the kernel's own dequantised operand and the
     standalone rotate kernel (both bit-checked elsewhere); ragged M (not a multiple of the token tile), merged
     projections, K longer than the weight ring (stage reuse), partial 128-column blocks."""
     import paroquant_b200.kernels.cuda  # noqa: F401
@@ -289,7 +289,7 @@ def test_group64_prepack_preserves_operand_bit_exact(PK, oracle, dt, K, parts):
 @pytest.mark.parametrize("dt", ["bfloat16", "float16"])
 @pytest.mark.parametrize("K,parts,Ms", [
     (512, [64], (1, 2, 5, 16, 17)),                   # cluster kernel, pre-rotated rows from 5 on, GEMM path at 17
-    (1024, [256, 128], (1, 4, 16, 48, 300)),          # merged; 48 / 300 rows: rotation pre-pass + tcgen05 GEMM
+    (1024, [256, 128], (1, 4, 16, 48, 300)),          # merged; 48 / 300 rows: rotation pre-pass + wgmma GEMM
     (640, [48, 16, 32], (3, 12)),
     (4096, [4096], (1, 16)),
 ])

@@ -1,10 +1,10 @@
-"""Same box, same inputs: our kernels against the UNMODIFIED reference pipeline (its rotate kernel
-from oracle/_ref + vLLM Marlin) executed in a separate process by tools/ref_gpu.py.
-Skipped when oracle/_ref was not built (it is built where /root/reference exists)."""
+"""Same inputs, our kernels against the UNMODIFIED reference pipeline (its rotate kernel + vLLM Marlin).
+
+The reference outputs are stored in tests/golden/ref_pipeline_samples.npz (tools/ref_gpu.py samples, run on an H100):
+for every seed-defined case the output's shape and a seeded sample of its elements (flat indices + raw bits).  The
+layer and the activations are regenerated here from the same seeds, our output is computed at full size and compared
+at the sampled elements: bit-exact for the rotation, relative error < 1e-3 for the fused linear."""
 import json
-import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -12,57 +12,35 @@ import torch
 
 from paroquant_b200.checkpoint import make_synthetic_activations, make_synthetic_layer
 
-ROOT = Path(__file__).resolve().parents[1]
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not (ROOT / "oracle" / "_ref" / "paroquant_rotation.so").exists(), reason="oracle/_ref not built")]
+from conftest import GOLDEN
 
-CASES = [
-    dict(name="rot_bf16", kind="rotate", dtype="bfloat16", M=16, K=4096, parts=[64], seed=1, xseed=2),
-    dict(name="rot_f16", kind="rotate", dtype="float16", M=3, K=4096, parts=[64], seed=3, xseed=4),
-    dict(name="rot_f32", kind="rotate", dtype="float32", M=5, K=1024, parts=[64], seed=5, xseed=6),
-    dict(name="o_m1", kind="linear", dtype="bfloat16", M=1, K=4096, parts=[4096], seed=7, xseed=8),
-    dict(name="o_m16", kind="linear", dtype="bfloat16", M=16, K=4096, parts=[4096], seed=7, xseed=9),
-    dict(name="qkv_m4", kind="linear", dtype="bfloat16", M=4, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=11),
-    dict(name="down_m1_f16", kind="linear", dtype="float16", M=1, K=14336, parts=[4096], seed=12, xseed=13),
-    # large M (rotation pre-pass + tcgen05 GEMM) at the batch sizes of BASELINE config 3, incl. K = 11008 / 14336
-    dict(name="o_m256", kind="linear", dtype="bfloat16", M=256, K=4096, parts=[4096], seed=7, xseed=14),
-    dict(name="o_m1024", kind="linear", dtype="bfloat16", M=1024, K=4096, parts=[4096], seed=7, xseed=15),
-    dict(name="qkv_m256", kind="linear", dtype="bfloat16", M=256, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=16),
-    dict(name="qkv_m1024", kind="linear", dtype="bfloat16", M=1024, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=17),
-    dict(name="l2down_m256", kind="linear", dtype="bfloat16", M=256, K=11008, parts=[4096], seed=18, xseed=19),
-    dict(name="l2down_m1024_f16", kind="linear", dtype="float16", M=1024, K=11008, parts=[4096], seed=18, xseed=20),
-    dict(name="down_m256", kind="linear", dtype="bfloat16", M=256, K=14336, parts=[4096], seed=12, xseed=21),
-    dict(name="down_m1024", kind="linear", dtype="bfloat16", M=1024, K=14336, parts=[4096], seed=12, xseed=22),
-    dict(name="gate_up_m16", kind="linear", dtype="bfloat16", M=16, K=4096, parts=[14336, 14336], seed=23, xseed=24),
-]
+pytestmark = pytest.mark.gpu
+
+_Z = np.load(GOLDEN / "ref_pipeline_samples.npz")
+CASES = json.loads(str(_Z["spec"]))
 _TD = {"float32": torch.float32, "float16": torch.float16, "bfloat16": torch.bfloat16}
 
 
-@pytest.fixture(scope="module")
-def ref_outputs(tmp_path_factory):
-    d = tmp_path_factory.mktemp("ref")
-    np.savez(d / "in.npz", spec=json.dumps(CASES))
-    r = subprocess.run([sys.executable, str(ROOT / "tools" / "ref_gpu.py"), "run", str(d / "in.npz"), str(d / "out.npz")],
-                       capture_output=True, text=True, timeout=1500)
-    if r.returncode:
-        pytest.skip(f"reference pipeline could not run here: {r.stderr[-400:]}")
-    return np.load(d / "out.npz")
-
-
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c["name"])
-def test_against_reference_kernels(ref_outputs, case):
+def test_against_reference_kernels(case):
     import paroquant_b200.kernels.cuda  # noqa: F401
     from paroquant_b200.linear import ParoLinearKernel
 
     dt = _TD[case["dtype"]]
     L = make_synthetic_layer(case["K"], case["parts"], seed=case["seed"]).to("cuda")
     x = make_synthetic_activations(case["M"], case["K"], seed=case["xseed"], dtype=dt).cuda()
-    ref = torch.from_numpy(np.ascontiguousarray(ref_outputs[case["name"]]))
+    name = case["name"]
+    idx = torch.from_numpy(_Z[name + "_idx"].astype(np.int64))
+    ref = torch.from_numpy(np.ascontiguousarray(_Z[name + "_val"]))
     ref = ref if dt == torch.float32 else ref.view(torch.int16).view(dt)
     if case["kind"] == "rotate":
         out = torch.ops.rotation.rotate(x, L.pairs[0], L.theta[0], L.channel_scales[0]).cpu()
-        assert torch.equal(out, ref), f"{(out != ref).float().mean().item():.4%} differ"   # bit exact
+        assert list(out.shape) == _Z[name + "_shape"].tolist()
+        got = out.reshape(-1)[idx]
+        assert torch.equal(got, ref), f"{(got != ref).float().mean().item():.4%} differ"   # bit exact
     else:
-        y = ParoLinearKernel.from_buffers(L, dt, check_pairs=False, max_m=case["M"])(x).float().cpu()
-        err = ((y - ref.float()).norm() / ref.float().norm()).item()
+        y = ParoLinearKernel.from_buffers(L, dt, check_pairs=False, max_m=case["M"])(x).cpu()
+        assert list(y.shape) == _Z[name + "_shape"].tolist()
+        got = y.reshape(-1)[idx].float()
+        err = ((got - ref.float()).norm() / ref.float().norm()).item()
         assert err < 1e-3, err

@@ -3,7 +3,7 @@ through the C-ABI.
 
 Three references:
   * tests/golden/ref_gpu_rotate_*.npz -- outputs of the UNMODIFIED reference kernel captured on a
-    B200: BIT-EXACT equality is required (same rounding points, same MUFU sin/cos);
+    H100: BIT-EXACT equality is required (same rounding points, same MUFU sin/cos);
   * the CPU oracle: identical except for MUFU vs correctly rounded sin/cos (bounded fraction of
     one-ulp flips);
   * size-independent properties at BASELINE sizes (theta = 0 identity, rotate / un-rotate

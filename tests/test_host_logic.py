@@ -120,7 +120,7 @@ def test_vllm_plugin_surface(vllm_plugin, monkeypatch):
     assert get_quantization_config("paroquant") is P.ParoQuantConfig
     cfg = P.ParoQuantConfig.from_config({"quant_method": "paroquant", "bits": 4, "group_size": 128, "krot": 8})
     assert (cfg.bits, cfg.group_size, cfg.krot, cfg.zero_point, cfg.pack_factor) == (4, 128, 8, True, 8)
-    assert cfg.get_name() == "paroquant" and cfg.get_min_capability() == 100
+    assert cfg.get_name() == "paroquant" and cfg.get_min_capability() == 90
     assert cfg.get_supported_act_dtypes() == [torch.half, torch.bfloat16]
     with pytest.raises(ValueError, match="Unsupported bits"):
         P.ParoQuantConfig(3, 128, 8, True)

@@ -1,6 +1,6 @@
 """CPU tests of the oracle itself: two independent restatements agree bit for bit, algebraic
 known-answer tests (SURVEY.md section 4), and -- when present -- the fixtures captured from the
-unmodified reference kernels on a B200 (tests/golden/ref_gpu_*.npz)."""
+unmodified reference kernels on an H100 (tests/golden/ref_gpu_*.npz)."""
 import numpy as np
 import pytest
 import torch

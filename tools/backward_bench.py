@@ -2,7 +2,7 @@
 backward STRUCTURE -- a Python walk over the rotations, per rotation two one-rotation rotate launches, gathers and a row
 reduction (/root/reference/paroquant/kernels/cuda/autograd.py:20-61) -- run on OUR rotate kernel, same box, CUDA events.
 
-    python tools/backward_bench.py [--out profiles/r02_backward_bench.json]
+    python tools/backward_bench.py [--out backward_bench.json]
 """
 import argparse
 import json

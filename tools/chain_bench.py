@@ -88,7 +88,7 @@ def main():
             return
         chains[0][0]()
         torch.cuda.synchronize()
-        nct, nst, nsl = 148, 6, 8
+        nct, nst, nsl = torch.cuda.get_device_properties(0).multi_processor_count, 6, 8
         buf = (ctypes.c_ulonglong * (nct * nst * nsl))()
         assert _cabi.lib().paro_debug_stream_trace(buf, nct) == 0
         t = torch.tensor(list(buf), dtype=torch.float64).view(nct, nst, nsl)

@@ -1,4 +1,4 @@
-"""Prefill microbenchmark (BASELINE.json config 2): fused rotate + dequant + tcgen05 GEMM,
+"""Prefill microbenchmark (BASELINE.json config 2): fused rotate + dequant + wgmma GEMM,
 batch in {256, 1024, 4096}, Llama shapes; TFLOP/s against the measured bf16 tensor roofline.
     python tools/gemm_bench.py [--out gpurun_out/gemm.json]
 """

@@ -7,7 +7,7 @@ Always a separate process: the reference library registers the same `rotation::r
 as paroquant_b200.kernels.cuda.  Nothing from paroquant_b200's kernels is imported here.
 
     python tools/ref_gpu.py golden  <outdir>          fixtures for tests/golden/
-    python tools/ref_gpu.py run     <in.npz> <out.npz> reference outputs for a test's inputs
+    python tools/ref_gpu.py samples <out.npz>         seeded samples of the outputs of PIPELINE_CASES (tests/test_gpu_reference.py)
     python tools/ref_gpu.py bench   <out.json> [--m 1,16,4096]  per-linear timings of rotate + Marlin (CUDA graph)
 """
 from __future__ import annotations
@@ -125,21 +125,48 @@ def golden(outdir: Path) -> None:
     print("golden fixtures written to", outdir)
 
 
-def run(inp: Path, out: Path) -> None:
-    """inputs: npz with seed-defined cases: arrays kind[], dtype[], M[], K[], parts (json), seeds."""
+# seed-defined cases of tests/test_gpu_reference.py: the layer and the activations are regenerated from the seeds there
+PIPELINE_CASES = [
+    dict(name="rot_bf16", kind="rotate", dtype="bfloat16", M=16, K=4096, parts=[64], seed=1, xseed=2),
+    dict(name="rot_f16", kind="rotate", dtype="float16", M=3, K=4096, parts=[64], seed=3, xseed=4),
+    dict(name="rot_f32", kind="rotate", dtype="float32", M=5, K=1024, parts=[64], seed=5, xseed=6),
+    dict(name="o_m1", kind="linear", dtype="bfloat16", M=1, K=4096, parts=[4096], seed=7, xseed=8),
+    dict(name="o_m16", kind="linear", dtype="bfloat16", M=16, K=4096, parts=[4096], seed=7, xseed=9),
+    dict(name="qkv_m4", kind="linear", dtype="bfloat16", M=4, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=11),
+    dict(name="down_m1_f16", kind="linear", dtype="float16", M=1, K=14336, parts=[4096], seed=12, xseed=13),
+    # large M (rotation pre-pass + tensor-core GEMM), incl. K = 11008 / 14336
+    dict(name="o_m256", kind="linear", dtype="bfloat16", M=256, K=4096, parts=[4096], seed=7, xseed=14),
+    dict(name="o_m1024", kind="linear", dtype="bfloat16", M=1024, K=4096, parts=[4096], seed=7, xseed=15),
+    dict(name="qkv_m256", kind="linear", dtype="bfloat16", M=256, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=16),
+    dict(name="qkv_m1024", kind="linear", dtype="bfloat16", M=1024, K=4096, parts=[4096, 1024, 1024], seed=10, xseed=17),
+    dict(name="l2down_m256", kind="linear", dtype="bfloat16", M=256, K=11008, parts=[4096], seed=18, xseed=19),
+    dict(name="l2down_m1024_f16", kind="linear", dtype="float16", M=1024, K=11008, parts=[4096], seed=18, xseed=20),
+    dict(name="down_m256", kind="linear", dtype="bfloat16", M=256, K=14336, parts=[4096], seed=12, xseed=21),
+    dict(name="down_m1024", kind="linear", dtype="bfloat16", M=1024, K=14336, parts=[4096], seed=12, xseed=22),
+    dict(name="gate_up_m16", kind="linear", dtype="bfloat16", M=16, K=4096, parts=[14336, 14336], seed=23, xseed=24),
+]
+SAMPLE_DRAWS = 4096   # seeded draws of flat indices per case; every 4th of them (sorted) is kept
+
+
+def samples(out: Path) -> None:
+    """Reference outputs of PIPELINE_CASES at a seeded sample of SAMPLE_DRAWS / 4 flat indices, as raw bits: small enough
+    to keep under tests/golden/."""
     rotate = load_reference_rotate()
-    spec = json.loads(str(np.load(inp)["spec"]))
-    res = {}
-    for c in spec:
+    res = {"spec": json.dumps(PIPELINE_CASES)}
+    for i, c in enumerate(PIPELINE_CASES):
         dt = _TD[c["dtype"]]
-        L = make_synthetic_layer(c["K"], c["parts"], seed=c["seed"], krot=c.get("krot", 8)).to("cuda")
+        L = make_synthetic_layer(c["K"], c["parts"], seed=c["seed"]).to("cuda")
         x = make_synthetic_activations(c["M"], c["K"], seed=c["xseed"], dtype=dt).to("cuda")
-        if c["kind"] == "rotate":
-            y = rotate(x, L.pairs[0], L.theta[0], L.channel_scales[0])
-        else:
-            y = ReferenceLinear(L, dt, rotate)(x)
-        res[c["name"]] = bits(y)
-    np.savez(out, **res)
+        y = rotate(x, L.pairs[0], L.theta[0], L.channel_scales[0]) if c["kind"] == "rotate" else ReferenceLinear(L, dt, rotate)(x)
+        flat = bits(y).reshape(-1)
+        n = min(flat.size, SAMPLE_DRAWS)
+        idx = np.sort(np.random.default_rng(1000 + i).choice(flat.size, n, replace=False))[::4].astype(np.int32)
+        res[c["name"] + "_shape"] = np.array(y.shape, dtype=np.int64)
+        res[c["name"] + "_idx"] = idx
+        res[c["name"] + "_val"] = flat[idx]
+    out.parent.mkdir(parents=True, exist_ok=True)
+    np.savez_compressed(out, **res)
+    print("reference samples written to", out)
 
 
 def bench(out: Path, ms: list[int]) -> None:
@@ -226,7 +253,7 @@ if __name__ == "__main__":
         sys.exit(0)
     if cmd == "golden":
         golden(Path(sys.argv[2]))
-    elif cmd == "run":
-        run(Path(sys.argv[2]), Path(sys.argv[3]))
+    elif cmd == "samples":
+        samples(Path(sys.argv[2]))
     elif cmd == "bench":
         bench(Path(sys.argv[2]), [int(v) for v in sys.argv[4].split(",")] if len(sys.argv) > 4 else [1])

@@ -24,11 +24,11 @@ from paroquant_b200.linear import ParoLinearKernel  # noqa: E402
 H, KV, I = 4096, 1024, 14336
 SH = {"o": (H, [H]), "gate_up": (H, [I, I]), "down": (I, [H]), "qkv": (H, [H, KV, KV])}
 NAMES = ["before pdl wait", "step start", "flag passed", "B operand ready", "first record", "rounds done", "epilogue done",
-         "last D read", "last D full", "last fix-up", "MMAs issued", "pass 1 start"]
+         "last D read", "last D full", "last fix-up", "-", "pass 1 start"]
 
 
 def dump(nsteps):
-    nct, nst, nsl = 148, 6, 12
+    nct, nst, nsl = torch.cuda.get_device_properties(0).multi_processor_count, 6, 12
     buf = (ctypes.c_ulonglong * (nct * nst * nsl))()
     assert _cabi.lib().paro_debug_stream_trace(buf, nct) == 0
     t = torch.tensor(list(buf), dtype=torch.float64).view(nct, nst, nsl)
