@@ -211,6 +211,10 @@ int paro_debug_decode_plan(const paro_linear_shape *shape, int64_t M, int32_t se
  * partition's team (+ end).                                                                                          */
 int paro_debug_stream_plan(const paro_linear_shape *shape, int64_t M, int32_t sets, int32_t ctas, int32_t *out);
 
+/* Test hook (host only): the tile of the M > 16 GEMM on a device with `sms` SMs.  out[0] = tokens per output tile (32, 64
+ * or 128), out[1] = token blocks (tiles along M; the last one is partial unless NT divides M).                       */
+int paro_debug_gemm_plan(const paro_linear_shape *shape, int64_t M, int32_t sms, int32_t *out);
+
 /* Developer aid: with PARO_DECODE_TRACE=1 the small-M kernel records, per CTA and step, 8 timestamps (SM cycles since
  * kernel entry).  Copies the first max_ctas x PARO_CHAIN_MAX_STEPS x 8 values of the last launch to host_out.        */
 int paro_debug_stream_trace(unsigned long long *host_out, int32_t max_ctas);

@@ -96,6 +96,8 @@ def lib() -> ctypes.CDLL:
         L.paro_tp_slot_bytes.argtypes = [shp, i64, i32]
         L.paro_debug_stream_plan.restype = ctypes.c_int
         L.paro_debug_stream_plan.argtypes = [shp, i64, i32, i32, ctypes.POINTER(ctypes.c_int32)]
+        L.paro_debug_gemm_plan.restype = ctypes.c_int
+        L.paro_debug_gemm_plan.argtypes = [shp, i64, i32, ctypes.POINTER(ctypes.c_int32)]
         L.paro_debug_stream_trace.restype = ctypes.c_int
         L.paro_debug_stream_trace.argtypes = [vp, i32]
         if L.paro_abi_version() != ABI_VERSION:
@@ -108,6 +110,7 @@ EXPORTED_SYMBOLS = (
     "paro_abi_version", "paro_last_error", "paro_last_launch_count", "paro_rotate", "paro_rotate_backward", "paro_packed_bytes",
     "paro_prepack", "paro_workspace_bytes", "paro_linear_forward", "paro_unpack_dense", "paro_debug_trace", "paro_debug_decode_plan",
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
+    "paro_debug_gemm_plan",
 )
 
 

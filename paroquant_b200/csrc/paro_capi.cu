@@ -48,6 +48,7 @@ int stream_linear_forward(const paro_linear_shape &s, const Layout &L, const voi
 int stream_trace_read(unsigned long long *host, int max_ctas);
 int stream_debug_plan(const Layout &L, int64_t M, int sets, int ctas, int32_t *out);
 size_t gemm_workspace_bytes(const Layout &L, int64_t max_m);
+int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out);
 int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
                  const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream);
 
@@ -200,6 +201,14 @@ int paro_debug_decode_plan(const paro_linear_shape *shape, int64_t M, int32_t se
   if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_decode_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
   if (!resident_clusters || !out || sms < 1) { set_error("debug_decode_plan: bad arguments"); return PARO_EINVAL; }
   return decode_debug_plan(L, M, sets, sms, resident_clusters, out);
+}
+
+int paro_debug_gemm_plan(const paro_linear_shape *shape, int64_t M, int32_t sms, int32_t *out) {
+  Layout L;
+  const char *why = "";
+  if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_gemm_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!out) { set_error("debug_gemm_plan: bad arguments"); return PARO_EINVAL; }
+  return gemm_debug_plan(L, M, sms, out);
 }
 
 static int chain_to_host(const paro_chain_step *steps, int32_t n, int64_t M, HostStep *hs) {

@@ -538,12 +538,12 @@ int decode_debug_plan(const Layout &L, int64_t M, int sets, int sms, const int32
 
 struct DecCached { bool found; DecPlan plan; DecSmem smem; };
 
+// the plan (cluster size, block ranges, shared-memory carve-up) depends on the shape, M and the device only: searched once
+// (the search asks the occupancy API and sets the function attribute), then looked up -- an eager launch is a map lookup
 template <typename T>
-static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t stream) {
+static DecCached dec_cached_plan(const Layout &L, int M, int sms) {
   auto kern = decode_kernel<T>;
   const DecKnobs &kn = dec_knobs();
-  // the plan (cluster size, block ranges, shared-memory carve-up) depends on the shape, M and the device only: searched once
-  // (the search asks the occupancy API and sets the function attribute), then looked up -- an eager launch is a map lookup
   struct Key {
     int K, N, krot, n_parts, M, dev, qhalves, parts[PARO_MAX_PARTS];
     bool operator<(const Key &o) const { return memcmp(this, &o, sizeof(Key)) < 0; }
@@ -552,7 +552,7 @@ static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t st
   static std::map<Key, DecCached> cache;
   Key key;
   memset(&key, 0, sizeof(key));
-  key.K = L.K; key.N = L.N; key.krot = L.krot; key.n_parts = L.n_parts; key.M = p.M; key.qhalves = L.qhalves;
+  key.K = L.K; key.N = L.N; key.krot = L.krot; key.n_parts = L.n_parts; key.M = M; key.qhalves = L.qhalves;
   if (cudaGetDevice(&key.dev) != cudaSuccess) key.dev = 0;
   for (int i = 0; i < L.n_parts; ++i) key.parts[i] = L.part_col_begin[i + 1] - L.part_col_begin[i];
   DecCached c;
@@ -561,7 +561,7 @@ static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t st
     auto it = cache.find(key);
     if (it == cache.end()) {
       DecCached fresh = {};
-      fresh.found = dec_choose_plan(L, p.M, p.rot_bytes, kDecSets, sms, !kn.no_cluster, kn.force_c,
+      fresh.found = dec_choose_plan(L, M, dec_rot_bytes(M), kDecSets, sms, !kn.no_cluster, kn.force_c,
                                     [&](int cc, int smem) { return max_resident_clusters<T>(cc, smem, sms); }, fresh.plan, fresh.smem);
       if (fresh.found && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) {
         (void)cudaGetLastError();
@@ -571,7 +571,13 @@ static int launch_decode(DecParams &p, const Layout &L, int sms, cudaStream_t st
     }
     c = it->second;
   }
-  if (!c.found) { set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, p.M); return PARO_EUNSUPPORTED; }
+  return c;
+}
+
+template <typename T>
+static int launch_decode(DecParams &p, const Layout &L, const DecCached &c, cudaStream_t stream) {
+  auto kern = decode_kernel<T>;
+  const DecKnobs &kn = dec_knobs();
   const DecPlan &best = c.plan;
   const DecSmem &best_s = c.smem;
   if (kn.verbose)
@@ -643,6 +649,10 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   static thread_local int sms_of[64] = {};   // SM count per device, asked once
   if (!sms_of[dev & 63]) PARO_CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
   const int sms = sms_of[dev & 63];
+  // no plan (e.g. K too long for one CTA without clusters): the caller falls back to the stream kernel, before any launch
+  const DecCached plan = s.dtype == PARO_BF16 ? dec_cached_plan<__nv_bfloat16>(L, static_cast<int>(M), sms)
+                                              : dec_cached_plan<__half>(L, static_cast<int>(M), sms);
+  if (!plan.found) { set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, static_cast<int>(M)); return PARO_EUNSUPPORTED; }
   const size_t part_bytes = static_cast<size_t>(kDecN) * L.K * 2;   // 16 rows (zero padded) x K of T, B-operand order
   const bool prerot = decode_wants_prerot(L, M) && scratch && scratch_bytes >= L.n_parts * part_bytes;
   if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_small_kernel)
@@ -667,7 +677,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   p.meta_group_bytes = L.meta_group_bytes;
   p.meta_off = static_cast<long long>(L.meta_off);
   p.rec_off = static_cast<long long>(L.rec_off);
-  return s.dtype == PARO_BF16 ? launch_decode<__nv_bfloat16>(p, L, sms, stream) : launch_decode<__half>(p, L, sms, stream);
+  return s.dtype == PARO_BF16 ? launch_decode<__nv_bfloat16>(p, L, plan, stream) : launch_decode<__half>(p, L, plan, stream);
 }
 
 }  // namespace paro

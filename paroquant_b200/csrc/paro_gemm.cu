@@ -201,12 +201,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
 // ~400 cycles of dequant per warpgroup: NT = 128 tiles keep the tensor pipe busy, but a small batch x few column blocks gives fewer
 // tiles than SMs (256 tokens x 4096 columns = 64 tiles) and is better cut finer -- pick the size with the shortest critical path
 // (waves x (rounds x max(dequant, MMA) + per-tile prologue / epilogue)).
-static int pick_nt(int64_t M, const Layout &L) {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
-  }
+// Pure host logic: `sms` is the device's SM count (tests drive it through paro_debug_gemm_plan).
+static int pick_nt(int64_t M, const Layout &L, int sms) {
   // from the largest tile the batch allows downwards: a finer tile must be CLEARLY better on paper (>= 25 %) -- finer tiles
   // re-read the weights more often and sit at the dequant limit, which the model prices optimistically
   int best = 0;
@@ -220,6 +216,24 @@ static int pick_nt(int64_t M, const Layout &L) {
     if (!best || t < 0.75 * best_t) { best = nt; best_t = t; }
   }
   return best;
+}
+
+static int gemm_device_sms() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
+  }
+  return sms;
+}
+
+// test hook: out[0] = tokens per tile (NT), out[1] = token blocks
+int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out) {
+  if (M < 1 || sms < 1) { set_error("debug_gemm_plan: bad M / sms"); return PARO_EINVAL; }
+  const int nt = pick_nt(M, L, sms);
+  out[0] = nt;
+  out[1] = static_cast<int32_t>((M + nt - 1) / nt);
+  return PARO_OK;
 }
 
 size_t gemm_workspace_bytes(const Layout &L, int64_t max_m) {
@@ -260,7 +274,7 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
     set_error("workspace too small: have %zu, need %zu", workspace_bytes, gemm_workspace_bytes(L, M));
     return PARO_EWORKSPACE;
   }
-  const int NT = pick_nt(M, L);
+  const int NT = pick_nt(M, L, gemm_device_sms());
   const int64_t m_pad = (M + NT - 1) / NT * NT;
   const uint8_t *pk = static_cast<const uint8_t *>(packed);
   uint8_t *xr_base = static_cast<uint8_t *>(workspace);

@@ -548,8 +548,11 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
           gs0 = gs1;
           const int Rp = g.blocks_p * ngs;
           const int lo = round_owner(jb * ngs, Rp, g.Tp), hi = round_owner((jb + 1) * ngs - 1, Rp, g.Tp);
-          if (sl == g.slice) myslot = total + (g.t - lo);
-          total += hi - lo + 1;
+          // a team with more members than rounds (Tp > Rp) has members without a round between lo and hi: then every round
+          // of the block has its own owner, who contributes slot (round - first round of the block)
+          const int n = hi - lo + 1 < ngs ? hi - lo + 1 : ngs;
+          if (sl == g.slice) myslot = total + (n < hi - lo + 1 ? ra - jb * ngs : g.t - lo);
+          total += n;
         }
         // the reducer: in slice (block mod c), the member that holds the block's last round there (spread over the slices)
         const bool reducer = static_cast<unsigned>(g.slice) == static_cast<unsigned>(gb) % static_cast<unsigned>(S.c) && rb == (jb + 1) * g.ng;
@@ -913,6 +916,8 @@ static bool stm_choose_plan(const Layout &L, int M, int sets, int ctas, int forc
         for (int s = 0; s < c; ++s) {
           const int ngs = (s + 1) * L.groups / c - s * L.groups / c;
           const int Rp = blocks * ngs;
+          // members lo..hi: an upper bound of the contributors the kernel counts (equal unless a team has more members than
+          // rounds); slots are sized and the plan is priced by it
           total += round_owner((jb + 1) * ngs - 1, Rp, Tp) - round_owner(jb * ngs, Rp, Tp) + 1;
         }
         if (total > pl.max_slots) pl.max_slots = total;

@@ -15,6 +15,7 @@ import torch
 from paroquant_b200.checkpoint import make_synthetic_activations, make_synthetic_layer
 
 from conftest import GOLDEN
+from gpu_reference import check_linear
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -69,23 +70,14 @@ def test_fused_linear_vs_oracle(PK, oracle, dt, K, parts, Ms):
 @pytest.mark.parametrize("K,parts", [(4096, [4096, 1024, 1024]), (4096, [14336, 14336]), (14336, [4096]), (11008, [4096])])
 def test_llama_shapes_vs_oracle_and_dense(PK, oracle, K, parts):
     """Llama-3-8B merged qkv / gate_up / down (+ Llama-2 K=11008 ragged slices) at M = 1 and 16:
-    column samples against the oracle, everything against a torch matmul on the kernel's own
-    dequantised operand and the standalone rotate kernel."""
-    import paroquant_b200.kernels.cuda  # noqa: F401
+    column samples against the oracle, every element against an fp64 matmul on the kernel's own
+    dequantised operand and the standalone rotate kernel (tests/gpu_reference.py)."""
     L = make_synthetic_layer(K, parts, seed=47, device="cuda")
     k = PK.from_buffers(L, torch.bfloat16)
-    W = k.dense_weight().float()
+    W = k.dense_weight()
     for M in (1, 16):
         x = make_synthetic_activations(M, K, seed=60 + M, device="cuda")
-        y = k(x).float()
-        n0, chunks = 0, []
-        for p, n in enumerate(parts):
-            xr = torch.ops.rotation.rotate(x, L.pairs[p], L.theta[p], L.channel_scales[p]).float()
-            chunks.append(xr.double() @ W[:, n0:n0 + n].double())
-            n0 += n
-        ref = torch.cat(chunks, -1).float().to(torch.bfloat16).double()   # same single final rounding
-        err = ((y.double() - ref).norm() / ref.norm()).item()
-        assert err < 3e-4, (M, err)                                        # only rare one-ulp flips remain
+        check_linear(k, L, x, k(x), W=W, what=f"M={M}")
     # oracle on a column sample (full oracle GEMM at these sizes would take minutes)
     cols = torch.arange(0, sum(parts), max(1, sum(parts) // 257))[:256]
     d = L.to("cpu").numpy_dict()
@@ -199,26 +191,15 @@ def test_vs_reference_pipeline_fixture(PK, path):
                                        (4096, [4096], 256), (4096, [4096, 1024, 1024], 300), (11008, [512], 33), (14336, [256], 257),
                                        (1152, [128], 40), (256, [272, 16], 33)])
 def test_large_m_gemm_vs_rotate_and_dense(PK, dt, K, parts, M):
-    """M > 16: rotation pre-pass + wgmma GEMM against fp64 matmul on the kernel's own dequantised operand and the
-    standalone rotate kernel (both bit-checked elsewhere); ragged M (not a multiple of the token tile), merged
-    projections, K longer than the weight ring (stage reuse), partial 128-column blocks."""
-    import paroquant_b200.kernels.cuda  # noqa: F401
+    """M > 16: rotation pre-pass + wgmma GEMM, every element against an fp64 matmul on the kernel's own dequantised operand
+    and the standalone rotate kernel (both bit-checked elsewhere; tests/gpu_reference.py); ragged M (not a multiple of the
+    token tile), merged projections, K longer than the weight ring (stage reuse), partial 128-column blocks."""
     L = make_synthetic_layer(K, parts, seed=53, device="cuda", bias=(M == 40))
     k = PK.from_buffers(L, _TD[dt], max_m=M)
-    W = k.dense_weight().double()
     x = make_synthetic_activations(M, K, seed=70 + M, device="cuda", dtype=_TD[dt])
     bias = None if L.bias is None else L.bias.to(_TD[dt])
     y = k(x, bias)
-    n0, chunks = 0, []
-    for p, n in enumerate(parts):
-        xr = torch.ops.rotation.rotate(x, L.pairs[p], L.theta[p], L.channel_scales[p]).double()
-        chunks.append(xr @ W[:, n0:n0 + n])
-        n0 += n
-    ref = torch.cat(chunks, -1).float().to(_TD[dt])
-    if bias is not None:
-        ref = (ref.float() + bias.float()).to(_TD[dt])
-    err = ((y.double() - ref.double()).norm() / ref.double().norm()).item()
-    assert err < 5e-4, err          # rare one-ulp flips of the final rounding (fp32 accumulation order over long K)
+    check_linear(k, L, x, y, bias, what=f"M={M}")
     assert torch.equal(k(x, bias), y)
 
 

@@ -53,7 +53,8 @@ def test_bit_exact_vs_reference_kernel_fixture(ops, path):
 
 
 @pytest.mark.parametrize("dt", ["bfloat16", "float16", "float32"])
-@pytest.mark.parametrize("M,K,G,krot", [(1, 4096, 128, 8), (16, 4096, 128, 8), (37, 1024, 128, 8), (9, 512, 64, 1), (5, 256, 64, 8)])
+@pytest.mark.parametrize("M,K,G,krot", [(1, 4096, 128, 8), (16, 4096, 128, 8), (37, 1024, 128, 8), (9, 512, 64, 1), (5, 256, 64, 8),
+                                         (4, 1024, 128, 2), (7, 512, 64, 3), (17, 1024, 128, 9), (3, 2048, 64, 16)])
 def test_vs_oracle(ops, oracle, dt, M, K, G, krot):
     L = make_synthetic_layer(K, [64], group_size=G, krot=krot, seed=21)
     x = make_synthetic_activations(M, K, seed=5, dtype=_TD[dt])

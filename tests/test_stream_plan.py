@@ -108,3 +108,53 @@ def test_bad_arguments():
     out = (ctypes.c_int32 * 16)()
     assert _cabi.lib().paro_debug_stream_plan(ctypes.byref(shape), 17, 5, 148, out) != 0
     assert _cabi.lib().paro_debug_stream_plan(ctypes.byref(shape), 1, 9, 148, out) != 0
+
+
+def deal_members(T, blocks):
+    """stm_deal_members: T members of a slice dealt to the partitions by 128-column blocks (largest remainder), >= 1 each."""
+    exact = [T * b / sum(blocks) for b in blocks]
+    alloc = [max(1, int(e)) for e in exact]
+    frac = [e - a for e, a in zip(exact, alloc)]
+    while sum(alloc) < T:
+        best = max(range(len(blocks)), key=lambda i: (frac[i], -i))
+        alloc[best] += 1
+        frac[best] -= 1
+    return [0] + [sum(alloc[:i + 1]) for i in range(len(blocks))]
+
+
+@pytest.mark.parametrize("K,parts", [(1024, [256, 128]), (512, [64]), (640, [48, 16, 32]), (2048, [384]), (4096, [4096, 1024, 1024])])
+@pytest.mark.parametrize("c", [1, 2, 3, 5, 8, 16])
+def test_forced_slices_count_only_members_with_rounds(K, parts, c):
+    """PARO_DECODE_C forces the number of K slices.  On a small layer a team then has more members than rounds, and members
+    without a round lie between the first and the last owner of a block's rounds: the kernel's seg table counts only the
+    owners (min(hi - lo + 1, ngs) per slice; a lone round's owner takes slot round - first round of the block).  Every block
+    must then get exactly `total` distinct slots below the planner's bound (the sum of hi - lo + 1), or its reducer waits
+    for ever."""
+    groups = K // 128
+    if c > groups:
+        pytest.skip("more slices than groups")
+    T = 132 // c
+    blocks = [(n + 127) // 128 for n in parts]
+    pcb = deal_members(T, blocks)
+    holes = False
+    for part, nb in enumerate(blocks):
+        Tp = pcb[part + 1] - pcb[part]
+        for jb in range(nb):
+            total = bound = 0
+            used = set()
+            for s in range(c):
+                ngs = (s + 1) * groups // c - s * groups // c
+                Rp = nb * ngs
+                lo, hi = round_owner(jb * ngs, Rp, Tp), round_owner((jb + 1) * ngs - 1, Rp, Tp)
+                n = min(hi - lo + 1, ngs)
+                holes |= n < hi - lo + 1
+                for t in range(Tp):                       # the members of slice s that own rounds of block jb
+                    r0, r1 = t * Rp // Tp, (t + 1) * Rp // Tp
+                    if max(r0, jb * ngs) < min(r1, (jb + 1) * ngs):
+                        used.add(total + (max(r0, jb * ngs) - jb * ngs if n < hi - lo + 1 else t - lo))
+                total += n
+                bound += hi - lo + 1
+            assert used == set(range(total)), (part, jb, sorted(used), total)
+            assert total <= bound
+    if (K, parts, c) == (1024, [256, 128], 3):
+        assert holes, "this case must exercise a team with more members than rounds"
