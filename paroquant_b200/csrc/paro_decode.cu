@@ -26,6 +26,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <type_traits>
 
 #include "paro_tc_common.cuh"
 
@@ -276,54 +277,79 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     DEC_TRACE(4);
 
     const int M = p.M;
-    const bool q2 = p.q2 != 0;
-    const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
     const int g = lane >> 2, t = lane & 3;
-    int st = 0;
-    uint32_t par = 0;
-    bool first = true;
+    const RoundLane lo = round_lane(p.q2 != 0, kDecN, tile, kh, lane);
+    const uint32_t ring_end = bar_wfull + 8 * NS;
+    // The round loop, specialised on the token tiles (NTT) and on tracing, so that neither is a per-round branch.  Stage
+    // and parity advance by increments: `fb` is the stage's full barrier, its empty barrier sits 8 * kDecMaxStages above.
+    auto rounds = [&](auto ntt, auto trace) {
+      constexpr int NTT = decltype(ntt)::value;
+      constexpr bool TRACE = decltype(trace)::value;
+      uint32_t fb = bar_wfull, rec = smem0, par = 0;
+      int tr = 0;   // rounds of CTA 0's per-round log written
 #pragma unroll 1
-    for (int j = 0; j < nj; ++j) {
-      float acc[2][4] = {};
+      for (int j = 0; j < nj; ++j) {
+        float acc[2][4] = {};
+        uint32_t xbg = xb;
 #pragma unroll 1
-      for (int gi = 0; gi < ng; ++gi) {
-        mbar_wait(bar_wfull + 8 * st, par);
-        if (first) { DEC_TRACE(5); first = false; }
-        const uint32_t rec = smem0 + st * rec_bytes, xbg = xb + gi * (kDecN * 256);
-        if (M > 8) mma_round<T, 2>(rec, q2, zero_off, xbg, kDecN, tile, kh, lane, acc);
-        else mma_round<T, 1>(rec, q2, zero_off, xbg, kDecN, tile, kh, lane, acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_wempty + 8 * st);
-        if (++st == NS) { st = 0; par ^= 1; }
-      }
-      // ---- block j closed: the k-half-1 warp hands its partial to its tile's k-half-0 warp, which adds it (fixed order)
-      // and stores or pushes the sum.  Two buffers by block parity: a warp writes buffer j & 1 again only after the pair
-      // barrier of block j + 1, which its partner reaches after reading it.
-      const uint32_t xc = xchg + ((j & 1) * 8 + tile) * (8 * 128) + lane * 4;
-      if (kh == 1) {
+        for (int gi = 0; gi < ng; ++gi) {
+          mbar_wait(fb, par);
+          if constexpr (TRACE) {
+            if (tr == 0) DEC_TRACE(5);
+            if (blockIdx.x == 0 && warp == 0 && lane == 0 && tr < 100)
+              g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * tr + 1] = clock64() - t_entry;   // seen full
+          }
+          mma_round<T, NTT>(rec, xbg, lo, kDecN, acc);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(fb + 8 * kDecMaxStages);
+          if constexpr (TRACE) {
+            if (blockIdx.x == 0 && warp == 0 && lane == 0 && tr < 100)
+              g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * tr + 2] = clock64() - t_entry;   // consumed
+            ++tr;
+          }
+          xbg += kDecN * 256;
+          fb += 8;
+          rec += rec_bytes;
+          if (fb == ring_end) { fb = bar_wfull; rec = smem0; par ^= 1; }
+        }
+        // ---- block j closed: the k-half-1 warp hands its partial to its tile's k-half-0 warp, which adds it (fixed order)
+        // and stores or pushes the sum.  Two buffers by block parity: a warp writes buffer j & 1 again only after the pair
+        // barrier of block j + 1, which its partner reaches after reading it.
+        const uint32_t xc = xchg + ((j & 1) * 8 + tile) * (8 * 128) + lane * 4;
+        if (kh == 1) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) sts_f32(xc + i * 128, acc[i >> 2][i & 3]);
-      }
-      named_bar_sync(4 + tile, 64);
-      if (kh == 0) {
+          for (int i = 0; i < 8; ++i) sts_f32(xc + i * 128, acc[i >> 2][i & 3]);
+        }
+        named_bar_sync(4 + tile, 64);
+        if (kh == 0) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] += lds_f32(xc + i * 128);
-        if (p.c > 1 && !cluster_ready) { cluster_wait_acquire(); cluster_ready = true; }  // #1: every peer CTA is running
-        const uint32_t dst = p.c > 1 ? map_to_rank(recv + (((j >> p.c_shift) << p.c_shift) + slice) * (M * 512), j & (p.c - 1)) : 0u;
+          for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] += lds_f32(xc + i * 128);
+          if (p.c > 1 && !cluster_ready) { cluster_wait_acquire(); cluster_ready = true; }  // #1: every peer CTA is running
+          const uint32_t dst = p.c > 1 ? map_to_rank(recv + (((j >> p.c_shift) << p.c_shift) + slice) * (M * 512), j & (p.c - 1)) : 0u;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int col = 16 * tile + g + 8 * ((i >> 1) & 1), m = 8 * (i >> 2) + 2 * t + (i & 1);
-          if (m < M) {
-            const float v = acc[i >> 2][i & 3];
-            if (p.c == 1) {
-              const int n = n_first + j * kBlockN + col;
-              if (n < n_end) dec_store<T>(p, v, m, n);
-            } else {
-              st_cluster_f32(dst + m * 512 + col * 4, v);
+          for (int i = 0; i < 8; ++i) {
+            const int col = 16 * tile + g + 8 * ((i >> 1) & 1), m = 8 * (i >> 2) + 2 * t + (i & 1);
+            if (m < M) {
+              const float v = acc[i >> 2][i & 3];
+              if (p.c == 1) {
+                const int n = n_first + j * kBlockN + col;
+                if (n < n_end) dec_store<T>(p, v, m, n);
+              } else {
+                st_cluster_f32(dst + m * 512 + col * 4, v);
+              }
             }
           }
         }
       }
+    };
+    using One = std::integral_constant<int, 1>;
+    using Two = std::integral_constant<int, 2>;
+    if (p.trace) {
+      if (M > 8) rounds(Two{}, std::true_type{});
+      else rounds(One{}, std::true_type{});
+    } else {
+      if (M > 8) rounds(Two{}, std::false_type{});
+      else rounds(One{}, std::false_type{});
     }
     DEC_TRACE(6);
   }

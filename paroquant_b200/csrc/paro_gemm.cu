@@ -40,20 +40,17 @@ struct GemmParams {
   long long rec_off, xr_part_stride;
 };
 
-// the A fragments of one round (8 k16 steps x 4 registers) for this warp's rows r and r + 8
+// the A fragments of one round (8 k16 steps x 4 registers) for this warp's 16-row tile: two 128-bit loads per lane
 template <typename T>
-__device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32_t zero_off, int r, int t, uint32_t (&a)[32]) {
-  RowDequant<T> d0, d1;
-  d0.prep(lds16(rec + kBlockScaleOff + 2 * r), lds8(rec + zero_off + r));
-  d1.prep(lds16(rec + kBlockScaleOff + 2 * (r + 8)), lds8(rec + zero_off + r + 8));
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    if (c == 2 && q2) {   // group_size 64: channels 64..127 of the record have their own scale / zero
-      d0.prep(lds16(rec + kBlockScaleOff + 256 + 2 * r), lds8(rec + zero_off + 128 + r));
-      d1.prep(lds16(rec + kBlockScaleOff + 256 + 2 * (r + 8)), lds8(rec + zero_off + 128 + r + 8));
-    }
-    frag_a2<T>(rec, r, c, t, d0, d1, *reinterpret_cast<uint32_t(*)[8]>(a + 8 * c));
-  }
+__device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32_t zero_off, int tile, int lane, uint32_t (&a)[32]) {
+  const int q = qparam_index(16 * tile + (lane >> 2));
+  const uint4 w0 = lds128(rec + frag_offset(tile, 0, lane)), w1 = lds128(rec + frag_offset(tile, 1, lane));
+  FragDequant<T> d;
+  d.prep(lds32(rec + kBlockScaleOff + 2 * q), lds16(rec + zero_off + q));
+  d.frag(w0.x, a + 0); d.frag(w0.y, a + 4); d.frag(w0.z, a + 8); d.frag(w0.w, a + 12);
+  if (q2)   // group_size 64: channels 64..127 of the record have their own scale / zero
+    d.prep(lds32(rec + kBlockScaleOff + 256 + 2 * q), lds16(rec + zero_off + 128 + q));
+  d.frag(w1.x, a + 16); d.frag(w1.y, a + 20); d.frag(w1.z, a + 24); d.frag(w1.w, a + 28);
 }
 
 template <typename T, int NT>
@@ -114,7 +111,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     // ================= consumers: warpgroup wg owns output columns 64 wg .. 64 wg + 63 of the block
     const int wg = (warp >> 2) - 1, w = warp & 3;
     const int g = lane >> 2, t = lane & 3;
-    const int r = 64 * wg + 16 * w + g;   // my rows r and r + 8 inside the block
+    const int tile = 4 * wg + w, r = 16 * tile + g;   // my 16-row tile, rows r and r + 8 inside the block
     const bool q2 = p.q2 != 0;
     const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
     const uint64_t desc_hi = smem_desc_kmajor(0, NT * 16, 128);
@@ -127,7 +124,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     auto dequant = [&](int rr, uint32_t (&a)[32]) {
       const int ws = rr % kWStages;
       mbar_wait(bar_wfull + 8 * ws, (rr / kWStages) & 1);
-      gemm_dequant_round<T>(w_ring + ws * kWStage, q2, zero_off, r, t, a);
+      gemm_dequant_round<T>(w_ring + ws * kWStage, q2, zero_off, tile, lane, a);
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_wempty + 8 * ws);
     };

@@ -9,17 +9,17 @@
 //   -> krot*256 + 256 bytes; lane l of the warp that owns the group reads 4 bytes of each row.
 //
 // Weight records.  N is cut into BLOCKS of 128 output columns per partition (a last partial block is
-// zero-filled), K into the quantisation groups of 128 channels.  One record = one (block, group) =
+// zero-filled), K into the quantisation groups of 128 channels.  One record = one (block, group gk) =
 // exactly what one dequant ROUND of either fused kernel consumes, and ONE cp.async.bulk (TMA) copy:
-//   weights  [t = 0..7][c = 0..3][row = 0..15] 16 bytes = 4 words; word j holds the 8 INT4 weights
-//            W[kb .. kb+7][n], n = 128*block + 16t + row, kb = 128*g + 32c + 8j, at bit positions
-//            0,16,4,20,8,24,12,28 -- so (w >> 4i) & 0x000F000F is the pair (kb+2i, kb+2i+1) sitting in
-//            the low mantissa bits of a bf16x2 / half2 word, i.e. one 32-bit register of an mma.sync / wgmma
-//            A fragment (row = output column n, channels kb+2i, kb+2i+1).
-//            One thread dequantises one COLUMN: 64 contiguous-in-k bytes per record, read as 4 x 16 B
-//            with the 16 rows of a chunk adjacent (conflict-free 128-bit shared loads).   (8192 bytes)
-//   scales   [128] T       s[g][n]                                                       (256 bytes)
-//   zeros    [128] uint8   z[g][n]                                                       (128 bytes)
+//   weights  [tile = 0..7][kh = 0..1][lane = 0..31] 16 bytes = 4 words: lane-private A fragments.  Word s is the whole
+//            mma.m16n8k16 A fragment of lane (g = lane / 4, t = lane % 4) for row tile `tile` and k16 step 4 kh + s:
+//            (w >> 4i) & 0x000F000F is register i, rows n = 128*block + 16*tile + g + 8*(i & 1), channels
+//            kb + 2t + 8*(i >> 1) (low half) and + 1 (high half), kb = 128*gk + 16*(4 kh + s) -- the pair sits in the low
+//            mantissa bits of a bf16x2 / half2 word.  A warp reads its (tile, k half) as one conflict-free 128-bit shared
+//            load per lane, 512 contiguous bytes; the wgmma GEMM's warps read both k halves.           (8192 bytes)
+//   scales   [128] T       s[gk][n], entry 16*tile + 2*g + hi for row 16*tile + g + 8*hi: a lane's two rows   (256 bytes)
+//            are one 32-bit word
+//   zeros    [128] uint8   z[gk][n], same order: a lane's two rows are one 16-bit word                        (128 bytes)
 // -> 8576 bytes.  group_size 64 (the converter rotates AND quantises in groups of `group_size`, cli/convert.py:176-182):
 // a record still covers 128 channels = TWO groups; it carries both groups' scales ([2][128] T at 8192) and then both
 // groups' zeros ([2][128] uint8) -> 8960 bytes; the pair indices of the second group are stored + 64, which makes the two
@@ -53,6 +53,10 @@ constexpr int kBlockBytes64 = 8192 + 512 + 256;    // group_size 64: two
 constexpr int kBlockBytesMax = kBlockBytes64;
 PARO_HD constexpr int block_bytes(int qhalves) { return kBlockWeightBytes + qhalves * 384; }
 PARO_HD constexpr int block_zero_off(int qhalves) { return kBlockScaleOff + qhalves * 256; }
+// byte offset of lane `lane`'s 16-byte A-fragment chunk of (row tile, k half) inside a record
+PARO_HD constexpr int frag_offset(int tile, int kh, int lane) { return ((tile * 2 + kh) * 32 + lane) * 16; }
+// entry of block column `col` (0..127) in a scale / zero set: rows g and g + 8 of a 16-row tile side by side
+PARO_HD constexpr int qparam_index(int col) { return (col & ~15) | ((col & 7) << 1) | ((col >> 3) & 1); }
 
 struct Layout {
   int K, N, krot, n_parts, dtype;

@@ -64,10 +64,6 @@ __global__ void prepack_meta_kernel(Layout L, const int16_t *__restrict__ pairs,
   rs[gk * kGroup + c] = csb;
 }
 
-// bit position of k-offset e (0..7) inside a word: consecutive k pairs land in the two 16-bit halves
-// so that (w >> 4i) & 0x000F000F is the bf16x2 / half2 payload of the A-fragment register of channel pair i of the word
-__device__ __constant__ int kNibblePos[8] = {0, 16, 4, 20, 8, 24, 12, 28};
-
 // block index over all partitions -> partition
 __device__ __forceinline__ int block_part(const Layout &L, int block) {
   int part = 0;
@@ -76,21 +72,24 @@ __device__ __forceinline__ int block_part(const Layout &L, int block) {
 }
 
 __global__ void prepack_weight_kernel(Layout L, const int32_t *__restrict__ qweight, uint8_t *__restrict__ packed) {
-  // one thread per output word: (record = (block, g), t, chunk c, row, j)
+  // one thread per output word: (record = (block, g), row tile, k half kh, lane, k16 step s of the half) -- paro_layout.h
   const int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   const int64_t total = static_cast<int64_t>(L.blocks_total) * L.groups * 2048;
   if (idx >= total) return;
-  const int j = idx & 3, row = (idx >> 2) & 15, c = (idx >> 6) & 3, t = (idx >> 8) & 7;
+  const int s = idx & 3, lane = (idx >> 2) & 31, kh = (idx >> 7) & 1, tile = (idx >> 8) & 7;
   const int64_t rec = idx >> 11;
   const int block = static_cast<int>(rec / L.groups), g = static_cast<int>(rec % L.groups);
   const int part = block_part(L, block);
-  const int n = L.part_col_begin[part] + (block - L.part_block_begin[part]) * kBlockN + t * 16 + row;
+  const int n0 = L.part_col_begin[part] + (block - L.part_block_begin[part]) * kBlockN + tile * 16 + (lane >> 2);
+  const int64_t k0 = static_cast<int64_t>(g) * kGroup + 16 * (4 * kh + s) + 2 * (lane & 3);
+  const int nc8 = L.N / 8;
   uint32_t w = 0;
-  if (n < L.part_col_begin[part + 1]) {
-    const int64_t kb = static_cast<int64_t>(g) * kGroup + 32 * c + 8 * j;
-    const int nc8 = L.N / 8;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) w |= awq_nibble(qweight, kb + e, n, nc8) << kNibblePos[e];
+  for (int i = 0; i < 4; ++i) {   // A-fragment register i: row g (+ 8 for odd i), channels 2t, 2t + 1 (+ 8 for i >= 2)
+    const int n = n0 + 8 * (i & 1);
+    const int64_t k = k0 + 8 * (i >> 1);
+    if (n < L.part_col_begin[part + 1])
+      w |= (awq_nibble(qweight, k, n, nc8) << (4 * i)) | (awq_nibble(qweight, k + 1, n, nc8) << (16 + 4 * i));
   }
   reinterpret_cast<uint32_t *>(packed + L.rec_off + rec * L.rec_bytes)[idx & 2047] = w;
 }
@@ -115,8 +114,8 @@ __global__ void prepack_qparam_kernel(Layout L, const int32_t *__restrict__ qzer
     z = static_cast<uint8_t>(awq_nibble(qzeros, qg, n, L.N / 8));
   }
   uint8_t *rb = packed + L.rec_off + rec * L.rec_bytes;
-  reinterpret_cast<uint16_t *>(rb + kBlockScaleOff)[h * 128 + col] = s;
-  rb[block_zero_off(L.qhalves) + h * 128 + col] = z;
+  reinterpret_cast<uint16_t *>(rb + kBlockScaleOff)[h * 128 + qparam_index(col)] = s;
+  rb[block_zero_off(L.qhalves) + h * 128 + qparam_index(col)] = z;
 }
 
 // Inverse, for tests: dense W[k][n] = T((q - z) * s_T), the exact operand the GEMM consumes.
@@ -130,15 +129,16 @@ __global__ void unpack_dense_kernel(Layout L, const uint8_t *__restrict__ packed
   while (n >= L.part_col_begin[part + 1]) ++part;
   const int nl = n - L.part_col_begin[part];
   const int block = L.part_block_begin[part] + nl / kBlockN, col = nl % kBlockN;
-  const int t = col >> 4, row = col & 15;
   const int g = k / kGroup, kl = k % kGroup;
-  const int c = kl >> 5, j = (kl >> 3) & 3, e = kl & 7;
+  // A-fragment position of (k, column): step kl / 16, lane (row % 8, channel pair), register (row / 8, channel / 8 of the step)
+  const int step = kl >> 4, kk = kl & 15, row = col & 15;
+  const int lane = 4 * (row & 7) + ((kk & 7) >> 1), i = (row >> 3) + 2 * (kk >> 3);
   const uint8_t *rb = packed + L.record_offset(block, g);
-  const uint32_t w = reinterpret_cast<const uint32_t *>(rb)[t * 256 + c * 64 + row * 4 + j];
-  const int q = (w >> kNibblePos[e]) & 0xF;
+  const uint32_t w = reinterpret_cast<const uint32_t *>(rb + frag_offset(col >> 4, step >> 2, lane))[step & 3];
+  const int q = (w >> (4 * i + 16 * (kk & 1))) & 0xF;
   const int h = L.qhalves == 2 ? kl >> 6 : 0;
-  const int z = rb[block_zero_off(L.qhalves) + h * 128 + col];
-  const T s = reinterpret_cast<const T *>(rb + kBlockScaleOff)[h * 128 + col];
+  const int z = rb[block_zero_off(L.qhalves) + h * 128 + qparam_index(col)];
+  const T s = reinterpret_cast<const T *>(rb + kBlockScaleOff)[h * 128 + qparam_index(col)];
   // (q - z) is exact in T; one rounding in the product, like the fused kernels
   W[idx] = Traits<T>::from_float(static_cast<float>(q - z) * Traits<T>::to_float(s));
 }

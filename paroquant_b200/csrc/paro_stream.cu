@@ -36,6 +36,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "paro_tc_common.cuh"
@@ -758,39 +759,52 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       if (wi == 0) STM_TRACE(i, 3);
       if (!g.active) continue;
 
-      const bool q2 = S.q2 != 0;
-      const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
+      const RoundLane lo = round_lane(S.q2 != 0, NR, tile, kh, lane);
       const SegWalk sw = seg_walk(g);
-      bool first = true;
-#pragma unroll 1
-      for (int k = 0; k < sw.nseg; ++k) {
-        int ra, rb;
-        seg_range(sw, k, ra, rb);
-        int gi = ra - static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng)) * g.ng;
-        float acc[2][4] = {};
-#pragma unroll 1
-        for (int r = ra; r < rb; ++r, ++gi) {
-          mbar_wait(bar_wfull + 8 * st, par);
-          if (first) { if (wi == 0) STM_TRACE(i, 4); first = false; }
-          const uint32_t rec = smem0 + st * p.stage_bytes, xbg = xb + gi * (NR * 256);
-          if (M > 8) mma_round<T, 2>(rec, q2, zero_off, xbg, NR, tile, kh, lane, acc);
-          else mma_round<T, 1>(rec, q2, zero_off, xbg, NR, tile, kh, lane, acc);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_wempty + 8 * st);
-          if (++st == NS) { st = 0; par ^= 1; }
-        }
-        // ---- segment done: my k half of the accumulator to the epilogue group
-        if (duse > 0) mbar_wait(bar_dfree + 8 * d, (duse - 1) & 1);
-        const uint32_t db = dbuf + d * dbuf_bytes + (kh * M) * 512;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int col = 16 * tile + g8 + 8 * ((e >> 1) & 1), m = 8 * (e >> 2) + 2 * t4 + (e & 1);
-          if (m < M) sts_f32(db + m * 512 + col * 4, acc[e >> 2][e & 3]);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_dfull + 8 * d);
-        if (++d == kStmDBufs) { d = 0; ++duse; }
+      if (p.trace && wi == 0 && sw.nseg > 0) {   // the step's first record has landed (waiting twice on one phase is harmless)
+        mbar_wait(bar_wfull + 8 * st, par);
+        STM_TRACE(i, 4);
       }
+      // The round loop, specialised on the token tiles so that M is no per-round branch; stage and parity advance by
+      // increments (`fb`: the stage's full barrier, its empty barrier sits 8 * kStmMaxStages above).
+      auto segments = [&](auto ntt) {
+        constexpr int NTT = decltype(ntt)::value;
+        const uint32_t ring_end = bar_wfull + 8 * NS;
+        uint32_t fb = bar_wfull + 8 * st, rec = smem0 + st * p.stage_bytes;
+#pragma unroll 1
+        for (int k = 0; k < sw.nseg; ++k) {
+          int ra, rb;
+          seg_range(sw, k, ra, rb);
+          const int gi = ra - static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng)) * g.ng;
+          uint32_t xbg = xb + gi * (NR * 256);
+          float acc[2][4] = {};
+#pragma unroll 1
+          for (int r = ra; r < rb; ++r) {
+            mbar_wait(fb, par);
+            mma_round<T, NTT>(rec, xbg, lo, NR, acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(fb + 8 * kStmMaxStages);
+            xbg += NR * 256;
+            fb += 8;
+            rec += p.stage_bytes;
+            if (fb == ring_end) { fb = bar_wfull; rec = smem0; par ^= 1; }
+          }
+          // ---- segment done: my k half of the accumulator to the epilogue group
+          if (duse > 0) mbar_wait(bar_dfree + 8 * d, (duse - 1) & 1);
+          const uint32_t db = dbuf + d * dbuf_bytes + (kh * M) * 512;
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            const int col = 16 * tile + g8 + 8 * ((e >> 1) & 1), m = 8 * (e >> 2) + 2 * t4 + (e & 1);
+            if (m < M) sts_f32(db + m * 512 + col * 4, acc[e >> 2][e & 3]);
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_dfull + 8 * d);
+          if (++d == kStmDBufs) { d = 0; ++duse; }
+        }
+        st = static_cast<int>((fb - bar_wfull) >> 3);
+      };
+      if (M > 8) segments(std::integral_constant<int, 2>{});
+      else segments(std::integral_constant<int, 1>{});
       if (wi == 0) STM_TRACE(i, 5);
     }
   }

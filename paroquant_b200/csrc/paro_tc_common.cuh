@@ -1,5 +1,5 @@
 // Device helpers shared by the tensor-core kernels (paro_decode.cu, paro_gemm.cu):
-// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T row dequant
+// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T A-fragment dequant
 // and the in-warp pairwise rotation (rounding points of /root/reference/paroquant/kernels/cuda/rotation.cuh:91-173).
 #pragma once
 #include "paro_common.cuh"
@@ -131,11 +131,6 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
   return v;
 }
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
-__device__ __forceinline__ uint32_t lds8(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ void sts128u(uint32_t addr, uint4 v) {
   asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
@@ -146,7 +141,7 @@ template <typename T> __device__ __forceinline__ T bits_to_T(uint32_t b) {
 }
 template <typename T> __device__ __forceinline__ uint16_t T_to_bits(T v) { return *reinterpret_cast<const uint16_t *>(&v); }
 
-// ------------------------------------------------------------------ INT4 -> T dequant of one row
+// ------------------------------------------------------------------ INT4 -> T dequant of A fragments
 // (a & mask) | magic in ONE LOP3: both constants must sit in registers (LOP3 takes one immediate)
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t mask, uint32_t magic) {
   uint32_t d;
@@ -154,70 +149,65 @@ __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t mask, uint32_t m
   return d;
 }
 
-template <typename T> struct RowDequant;
-
-template <> struct RowDequant<__nv_bfloat16> {
-  uint32_t s2, z2;
-  __device__ __forceinline__ void prep(uint32_t s_bits, uint32_t z) {
-    s2 = s_bits * 0x00010001u;
-    z2 = (0x4300u | z) * 0x00010001u;  // bf16x2 {128 + z, 128 + z}
-  }
-  __device__ __forceinline__ uint32_t one(uint32_t w) const {
-    // 0x4300 | q is the bf16 128 + q; (128 + q) - (128 + z) is exact; one rounding in the multiply
-    const __nv_bfloat162 d = __hsub2(unpack2<__nv_bfloat16>(and_or(w, 0x000F000Fu, 0x43004300u)), unpack2<__nv_bfloat16>(z2));
-    return pack2<__nv_bfloat16>(__hmul2(d, unpack2<__nv_bfloat16>(s2)));
-  }
-  // pair t (channels 2t, 2t + 1) of a record word
-  __device__ __forceinline__ uint32_t pair(uint32_t w, int t) const { return one(w >> (4 * t)); }
-};
-
-template <> struct RowDequant<__half> {
-  uint32_t s2, z_lo;
-  __device__ __forceinline__ void prep(uint32_t s_bits, uint32_t z) {
-    s2 = s_bits * 0x00010001u;
-    z_lo = (0x6400u | z) * 0x00010001u;   // {1024 + z}
-  }
-  // 0x6400 | q = 1024 + q; (1024 + q) - (1024 + z) = q - z exactly, one rounding in the multiply
-  __device__ __forceinline__ uint32_t pair(uint32_t w, int t) const {
-    return pack2<__half>(__hmul2(__hsub2(unpack2<__half>(and_or(w >> (4 * t), 0x000F000Fu, 0x64006400u)), unpack2<__half>(z_lo)), unpack2<__half>(s2)));
-  }
-};
-
-// A fragments of k16 steps 2c and 2c + 1 (channels 32c .. 32c + 31 of a record) for rows r and r + 8 of a 16-row tile
-// (r = 16 * tile + lane / 4): one 128-bit load per row -- the four lanes of a row read the same 16 bytes (paro_layout.h:
-// word j of a chunk holds channels 8j .. 8j + 7), each keeps its pair t = lane % 4 of every word.
+// Dequantiser of one lane's rows g and g + 8 of a 16-row tile (paro_layout.h: the two rows' scales are one 32-bit word of
+// the record, their zeros one 16-bit word).  magic | q is the T value base + q (bf16 0x4300 = 128, half 0x6400 = 1024):
+// (base + q) - (base + z) = q - z exactly, then one rounding in the multiply by the scale.
 template <typename T>
-__device__ __forceinline__ void frag_a2(uint32_t rec, int r, int c, int t, const RowDequant<T> &d0, const RowDequant<T> &d1, uint32_t (&a)[8]) {
-  const uint32_t base = rec + (r >> 4) * 1024 + c * 256 + (r & 15) * 16;
-  const uint4 w0 = lds128(base), w1 = lds128(base + 128);
-  a[0] = d0.pair(w0.x, t); a[1] = d1.pair(w1.x, t); a[2] = d0.pair(w0.y, t); a[3] = d1.pair(w1.y, t);
-  a[4] = d0.pair(w0.z, t); a[5] = d1.pair(w1.z, t); a[6] = d0.pair(w0.w, t); a[7] = d1.pair(w1.w, t);
+struct FragDequant {
+  static constexpr uint32_t kMagic = Traits<T>::code == PARO_BF16 ? 0x43004300u : 0x64006400u;
+  uint32_t s0, s1, z0, z1;   // T x2 {s, s} and {base + z, base + z} of rows g (0) and g + 8 (1)
+  __device__ __forceinline__ void prep(uint32_t s_pair, uint32_t z_pair) {
+    s0 = __byte_perm(s_pair, 0u, 0x1010);
+    s1 = __byte_perm(s_pair, 0u, 0x3232);
+    z0 = __byte_perm(z_pair, kMagic >> 8, 0x4040);   // bytes {z, magic byte, z, magic byte}
+    z1 = __byte_perm(z_pair, kMagic >> 8, 0x4141);
+  }
+  __device__ __forceinline__ uint32_t one(uint32_t w, uint32_t z, uint32_t sc) const {
+    using T2 = typename Traits<T>::T2;
+    const T2 d = __hsub2(unpack2<T>(and_or(w, 0x000F000Fu, kMagic)), unpack2<T>(z));
+    return pack2<T>(__hmul2(d, unpack2<T>(sc)));
+  }
+  // the A fragment of one k16 step from its record word: register i = (w >> 4i) & 0x000F000F, rows g / g + 8 alternating
+  __device__ __forceinline__ void frag(uint32_t w, uint32_t *a) const {
+    a[0] = one(w, z0, s0);
+    a[1] = one(w >> 4, z1, s1);
+    a[2] = one(w >> 8, z0, s0);
+    a[3] = one(w >> 12, z1, s1);
+  }
+};
+
+// Per-lane shared-memory offsets of a small-M worker warp's round: they depend on the warp's (tile, k half) and the lane
+// only, so the round loop computes them once.  w / s / z are record-relative, x is relative to the group's B operand.
+struct RoundLane {
+  uint32_t w, s, z, x;
+};
+__device__ __forceinline__ RoundLane round_lane(bool q2, int NR, int tile, int kh, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const bool second = q2 && kh;   // group_size 64: channels 64..127 (kh = 1) have the record's second scale / zero set
+  RoundLane o;
+  o.w = frag_offset(tile, kh, lane);
+  o.s = kBlockScaleOff + (second ? 256 : 0) + 2 * qparam_index(16 * tile + g);
+  o.z = block_zero_off(q2 ? 2 : 1) + (second ? 128 : 0) + qparam_index(16 * tile + g);
+  o.x = 4 * kh * (NR * 32) + g * 16 + t * 4;
+  return o;
 }
 
 // One record (128 columns x 128 channels) of a small-M worker warp: its 16-row tile, k16 steps 4 kh .. 4 kh + 3, NTT token
 // tiles of 8.  B (x_rot of the record's group) is K-major core matrices: [k16 step][k half][row / 8][row % 8][8 elements],
-// NR rows per step (8 or 16).  group_size 64: channels 64..127 (kh = 1) have the record's second scale / zero set.
+// NR rows per step (8 or 16).  One 128-bit load brings the lane's four A fragments (paro_layout.h).
 template <typename T, int NTT>
-__device__ __forceinline__ void mma_round(uint32_t rec, bool q2, uint32_t zero_off, uint32_t xbg, int NR, int tile, int kh, int lane, float (&acc)[2][4]) {
-  const int g = lane >> 2, t = lane & 3, r = 16 * tile + g;
-  const uint32_t so = (q2 && kh) ? 256 : 0, zo = (q2 && kh) ? 128 : 0;
-  RowDequant<T> d0, d1;
-  d0.prep(lds16(rec + kBlockScaleOff + so + 2 * r), lds8(rec + zero_off + zo + r));
-  d1.prep(lds16(rec + kBlockScaleOff + so + 2 * (r + 8)), lds8(rec + zero_off + zo + r + 8));
+__device__ __forceinline__ void mma_round(uint32_t rec, uint32_t xbg, const RoundLane &o, int NR, float (&acc)[2][4]) {
+  FragDequant<T> d;
+  d.prep(lds32(rec + o.s), lds16(rec + o.z));
+  const uint4 w = lds128(rec + o.w);
+  const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-  for (int cc = 0; cc < 2; ++cc) {
-    const int c = 2 * kh + cc;
-    uint32_t a[8];
-    frag_a2<T>(rec, r, c, t, d0, d1, a);
+  for (int s = 0; s < 4; ++s) {
+    uint32_t a[4];
+    d.frag(ws[s], a);
+    const uint32_t bs = xbg + o.x + s * (NR * 32);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const uint32_t bs = xbg + (2 * c + h) * (NR * 32) + t * 4;
-#pragma unroll
-      for (int nt = 0; nt < NTT; ++nt) {
-        const uint32_t ba = bs + nt * 128 + g * 16;
-        mma16816<T>(acc[nt], a + 4 * h, lds32(ba), lds32(ba + NR * 16));
-      }
-    }
+    for (int nt = 0; nt < NTT; ++nt) mma16816<T>(acc[nt], a, lds32(bs + nt * 128), lds32(bs + nt * 128 + NR * 16));
   }
 }
 
