@@ -442,6 +442,7 @@ __device__ __forceinline__ void stm_prologue(const StepDesc &S, int M, int NR, R
 template <typename T, int SETS, int MB>
 __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __grid_constant__ StreamParams p) {
   static_assert(SETS == 4, "the workers are 8 row tiles x 2 k halves");
+  static_assert(SETS % 2 == 0, "the ring depth is a multiple of SETS; the round loop takes records in pairs that must not wrap");
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int kWorkers = 4 * SETS;
   constexpr int kEpiWarp0 = kWorkers, kProdWarp = kWorkers + 4;
@@ -759,36 +760,51 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       if (wi == 0) STM_TRACE(i, 3);
       if (!g.active) continue;
 
-      const RoundLane lo = round_lane(S.q2 != 0, NR, tile, kh, lane);
       const SegWalk sw = seg_walk(g);
       if (p.trace && wi == 0 && sw.nseg > 0) {   // the step's first record has landed (waiting twice on one phase is harmless)
         mbar_wait(bar_wfull + 8 * st, par);
         STM_TRACE(i, 4);
       }
-      // The round loop, specialised on the token tiles so that M is no per-round branch; stage and parity advance by
-      // increments (`fb`: the stage's full barrier, its empty barrier sits 8 * kStmMaxStages above).
-      auto segments = [&](auto ntt) {
-        constexpr int NTT = decltype(ntt)::value;
-        const uint32_t ring_end = bar_wfull + 8 * NS;
-        uint32_t fb = bar_wfull + 8 * st, rec = smem0 + st * p.stage_bytes;
+      // The round loop, specialised on the token tiles and the B rows so that neither is a per-round branch or multiply;
+      // stage and parity advance by increments (`fb`: the stage's full barrier, its empty barrier sits 8 * kStmMaxStages
+      // above).  Records are taken in pairs from an even stage: the ring depth is a multiple of SETS (even), so a pair
+      // never wraps.  A segment starting at an odd stage takes its first record alone, an odd remainder its last.
+      auto segments = [&](auto ntt, auto nr) {
+        constexpr int NTT = decltype(ntt)::value, NRC = decltype(nr)::value;
+        const RoundLane lo = round_lane<NRC>(S.q2 != 0, tile, kh, lane);
+        const uint32_t ring_end = bar_wfull + 8 * NS, stage_bytes = p.stage_bytes;
+        // a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * stage_bytes (a multiple of 8)
+        const uint32_t rec_per_bar = stage_bytes / 8, rec_at_bar0 = smem0 - bar_wfull * rec_per_bar;
+        uint32_t fb = bar_wfull + 8 * st, bx;   // bx: this lane's ldmatrix row in the B operand of the next group
+        float acc[2][4];
+        auto take = [&](auto nrec) {
+          constexpr int NREC = decltype(nrec)::value;
+#pragma unroll
+          for (int i = 0; i < NREC; ++i) mbar_wait(fb + 8 * i, par);
+          mma_rounds<T, NTT, NREC, NRC>(fb * rec_per_bar + rec_at_bar0, stage_bytes, bx, lo, acc);
+          __syncwarp();
+          if (elect_one()) {
+#pragma unroll
+            for (int i = 0; i < NREC; ++i) mbar_arrive(fb + 8 * i + 8 * kStmMaxStages);
+          }
+          bx += NREC * (NRC * 256);
+          fb += 8 * NREC;
+          if (fb == ring_end) { fb = bar_wfull; par ^= 1; }
+        };
 #pragma unroll 1
         for (int k = 0; k < sw.nseg; ++k) {
           int ra, rb;
           seg_range(sw, k, ra, rb);
           const int gi = ra - static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng)) * g.ng;
-          uint32_t xbg = xb + gi * (NR * 256);
-          float acc[2][4] = {};
+          bx = xb + gi * (NRC * 256) + lo.x;
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[e >> 2][e & 3] = 0.f;
+          int left = rb - ra;
+          if (left > 0 && ((fb - bar_wfull) & 8)) { take(std::integral_constant<int, 1>{}); --left; }
+          const uint32_t pairs_end = bx + (left >> 1) * (2 * NRC * 256);   // the pair loop counts with bx
 #pragma unroll 1
-          for (int r = ra; r < rb; ++r) {
-            mbar_wait(fb, par);
-            mma_round<T, NTT>(rec, xbg, lo, NR, acc);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(fb + 8 * kStmMaxStages);
-            xbg += NR * 256;
-            fb += 8;
-            rec += p.stage_bytes;
-            if (fb == ring_end) { fb = bar_wfull; rec = smem0; par ^= 1; }
-          }
+          while (bx != pairs_end) take(std::integral_constant<int, 2>{});
+          if (left & 1) take(std::integral_constant<int, 1>{});
           // ---- segment done: my k half of the accumulator to the epilogue group
           if (duse > 0) mbar_wait(bar_dfree + 8 * d, (duse - 1) & 1);
           const uint32_t db = dbuf + d * dbuf_bytes + (kh * M) * 512;
@@ -803,8 +819,11 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
         }
         st = static_cast<int>((fb - bar_wfull) >> 3);
       };
-      if (M > 8) segments(std::integral_constant<int, 2>{});
-      else segments(std::integral_constant<int, 1>{});
+      using I1 = std::integral_constant<int, 1>;
+      using I2 = std::integral_constant<int, 2>;
+      if (M > 8) segments(I2{}, std::integral_constant<int, 16>{});
+      else if (NR == 8) segments(I1{}, std::integral_constant<int, 8>{});
+      else segments(I1{}, std::integral_constant<int, 16>{});
       if (wi == 0) STM_TRACE(i, 5);
     }
   }

@@ -176,38 +176,63 @@ struct FragDequant {
   }
 };
 
+// four 8 x 8 b16 matrices; lanes 8i .. 8i + 7 give the row addresses of matrix i, register i of lane l holds its row
+// l / 4, elements 2 (l % 4) and + 1 -- for a K-major core matrix that is an mma.m16n8k16 .col B fragment register
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+
 // Per-lane shared-memory offsets of a small-M worker warp's round: they depend on the warp's (tile, k half) and the lane
-// only, so the round loop computes them once.  w / s / z are record-relative, x is relative to the group's B operand.
+// only, so the round loop computes them once.  w / s / z are record-relative, x is relative to the group's B operand:
+// the row this lane hands to ldmatrix.x4 for k16 steps (4 kh, 4 kh + 1) -- matrices {step, k half} = {0, 0}, {0, 1},
+// {1, 0}, {1, 1}, i.e. b0, b1 of the first step and b0, b1 of the second.
 struct RoundLane {
   uint32_t w, s, z, x;
 };
-__device__ __forceinline__ RoundLane round_lane(bool q2, int NR, int tile, int kh, int lane) {
-  const int g = lane >> 2, t = lane & 3;
+template <int NR>
+__device__ __forceinline__ RoundLane round_lane(bool q2, int tile, int kh, int lane) {
+  const int g = lane >> 2;
   const bool second = q2 && kh;   // group_size 64: channels 64..127 (kh = 1) have the record's second scale / zero set
   RoundLane o;
   o.w = frag_offset(tile, kh, lane);
   o.s = kBlockScaleOff + (second ? 256 : 0) + 2 * qparam_index(16 * tile + g);
   o.z = block_zero_off(q2 ? 2 : 1) + (second ? 128 : 0) + qparam_index(16 * tile + g);
-  o.x = 4 * kh * (NR * 32) + g * 16 + t * 4;
+  o.x = (4 * kh + (lane >> 4)) * (NR * 32) + ((lane >> 3) & 1) * (NR * 16) + (lane & 7) * 16;
   return o;
 }
 
-// One record (128 columns x 128 channels) of a small-M worker warp: its 16-row tile, k16 steps 4 kh .. 4 kh + 3, NTT token
-// tiles of 8.  B (x_rot of the record's group) is K-major core matrices: [k16 step][k half][row / 8][row % 8][8 elements],
-// NR rows per step (8 or 16).  One 128-bit load brings the lane's four A fragments (paro_layout.h).
-template <typename T, int NTT>
-__device__ __forceinline__ void mma_round(uint32_t rec, uint32_t xbg, const RoundLane &o, int NR, float (&acc)[2][4]) {
-  FragDequant<T> d;
-  d.prep(lds32(rec + o.s), lds16(rec + o.z));
-  const uint4 w = lds128(rec + o.w);
-  const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+// NREC (1 or 2) records of consecutive groups for a small-M worker warp: record i at rec + i * rec_stride, its B operand
+// (x_rot of the group) at bx - o.x + i * NR * 256, where bx is this lane's ldmatrix row of the first group.  Per record the
+// warp takes its 16-row tile, k16 steps 4 kh .. 4 kh + 3, NTT token tiles of 8.  B is K-major core matrices: [k16 step]
+// [k half][row / 8][row % 8][8 elements], NR rows per step (8 or 16).  One 128-bit load brings a record's four A fragments
+// (paro_layout.h), two ldmatrix.x4 its B fragments per token tile.  Every load of both records is issued first and the two
+// dequants are independent, so one ring wait covers two records' worth of latency; the MMAs go into ONE accumulator in
+// record, step order -- the sum order of one record per call, so the result does not depend on how records are paired.
+template <typename T, int NTT, int NREC, int NR>
+__device__ __forceinline__ void mma_rounds(uint32_t rec, uint32_t rec_stride, uint32_t bx, const RoundLane &o, float (&acc)[2][4]) {
+  FragDequant<T> d[NREC];
+  uint4 w[NREC];
+  uint32_t b[NREC][NTT][2][4];   // [record][token tile][steps 0-1 / 2-3][b0, b1 of the first step, b0, b1 of the second]
 #pragma unroll
-  for (int s = 0; s < 4; ++s) {
-    uint32_t a[4];
-    d.frag(ws[s], a);
-    const uint32_t bs = xbg + o.x + s * (NR * 32);
+  for (int i = 0; i < NREC; ++i) {
+    const uint32_t r = rec + i * rec_stride;
+    d[i].prep(lds32(r + o.s), lds16(r + o.z));
+    w[i] = lds128(r + o.w);
 #pragma unroll
-    for (int nt = 0; nt < NTT; ++nt) mma16816<T>(acc[nt], a, lds32(bs + nt * 128), lds32(bs + nt * 128 + NR * 16));
+    for (int nt = 0; nt < NTT; ++nt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) ldsm_x4(bx + i * (NR * 256) + h * (NR * 64) + nt * 128, b[i][nt][h]);
+  }
+#pragma unroll
+  for (int i = 0; i < NREC; ++i) {
+    const uint32_t ws[4] = {w[i].x, w[i].y, w[i].z, w[i].w};
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      uint32_t a[4];
+      d[i].frag(ws[s], a);
+#pragma unroll
+      for (int nt = 0; nt < NTT; ++nt) mma16816<T>(acc[nt], a, b[i][nt][s >> 1][2 * (s & 1)], b[i][nt][s >> 1][2 * (s & 1) + 1]);
+    }
   }
 }
 

@@ -7,7 +7,7 @@ Each shape is timed over enough distinct weight sets to exceed the 50 MB L2 (>= 
 CUDA graph of back-to-back launches (PDL on), CUDA events around several replays.  --sets 1 cycles one
 weight set that stays in L2 instead (graph of the same length): the kernel's own cost per record without
 the HBM stream.  Streaming time close to the L2-resident time means the consumer round, not HBM, is the limit.
-Environment knobs forwarded to the library: PARO_DECODE_STAGES, PARO_DECODE_CTAS_PER_SM, PARO_NO_PDL.
+Environment knobs forwarded to the library: PARO_DECODE_STAGES, PARO_NO_PDL.
 """
 from __future__ import annotations
 
