@@ -23,6 +23,8 @@
  *                            per partition, cat, bias) and RotateQuantizedLinear.forward
  *                            paroquant/inference/backends/transformers/modules.py:57-71
  *   paro_last_error        TORCH_CHECK messages of rotation.cu:66,92,108,114,123
+ *   paro_moe_forward       RotateSwitchGLU  paroquant/inference/backends/mlx/modules.py:159-212 on the
+ *                            expert format of paroquant/cli/convert.py:281-406
  *
  * Return value of every int function: 0 on success, a PARO_E* code otherwise; the message is
  * available from paro_last_error() on the same thread.
@@ -37,7 +39,7 @@
 extern "C" {
 #endif
 
-#define PARO_ABI_VERSION 3
+#define PARO_ABI_VERSION 4
 #define PARO_MAX_PARTS 8
 
 /* element types (activations, rotation parameters, scales) */
@@ -189,6 +191,47 @@ size_t paro_chain_workspace_bytes(const paro_chain_step *steps, int32_t n_steps,
 /* Run the chain for M <= 16 rows.  One launch; CUDA-graph safe; no allocation, no host synchronisation.             */
 int paro_chain_forward(const paro_chain_step *steps, int32_t n_steps, int64_t M, void *workspace,
                        size_t workspace_bytes, paro_stream_t stream);
+
+/* ---- MoE expert block for decode batches: the routed experts of one block in TWO launches, routing read on the device ----
+ * Replaces the reference's RotateSwitchGLU (paroquant/inference/backends/mlx/modules.py:159-212) on the expert format of
+ * paroquant/cli/convert.py:281-406: every expert is a merged gate|up linear and a down linear, and all experts share ONE
+ * gate_up rotation and ONE down rotation.  For token t and slot s with e = topk_ids[t, s] in [0, n_experts):
+ *   h[t, s]  = T(rotate_gu(x[t]) . W_gu[e])                              (2I outputs: gate | up)
+ *   y_s      = T(rotate_d(T(T(silu(gate)) * up)) . W_d[e])
+ *   y[t]     = T(sum of fp32(y_s) * w_s, from 0, in ascending (expert id, slot) order, each product rounded before its add)
+ * A slot whose id lies outside [0, n_experts) contributes nothing (expert parallelism marks non-local experts with -1);
+ * duplicate ids in one token each contribute.  Two PDL-chained launches, no host synchronisation, no allocation; one
+ * launch plan serves every routing, so a captured CUDA graph stays valid while the ids / weights in its buffers change.  */
+typedef struct paro_moe_desc {
+  const paro_linear_shape *gate_up;  /* every expert's merged gate|up: in_features = hidden, parts {I, I}               */
+  const paro_linear_shape *down;     /* every expert's down: in_features = I, parts {hidden}                            */
+  int32_t n_experts;
+  const void *gate_up_packed;        /* device; expert e's paro_prepack buffer at + e * gate_up_stride                  */
+  size_t gate_up_stride;             /* >= paro_packed_bytes(gate_up), multiple of 256                                  */
+  const void *down_packed;
+  size_t down_stride;
+} paro_moe_desc;
+
+/* Workspace bytes for paro_moe_forward (0 on an invalid descriptor or batch).                                          */
+size_t paro_moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t top_k);
+
+/* Run the expert block for T tokens with top_k slots each.
+ *   x             device [T, hidden] of the shapes' dtype
+ *   topk_ids      device [T, top_k] int32;  topk_weights device [T, top_k] fp32
+ *   h             device [T, top_k, 2I]: the gate|up outputs (rows of dropped slots are left unspecified)
+ *   y             device [T, hidden]
+ * 1 <= T <= 16, 1 <= top_k <= 16 and T * top_k <= 128 (the routing table is built by one thread per entry in shared
+ * memory); otherwise PARO_EUNSUPPORTED.  paro_last_launch_count() reports 2.                                          */
+int paro_moe_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_ids, const float *topk_weights,
+                     int64_t T, int32_t top_k, void *h, void *y, void *workspace, size_t workspace_bytes,
+                     paro_stream_t stream);
+
+/* Test hook (host only): the two launch plans of paro_moe_forward on a device with `sms` SMs and a walk of their work
+ * lists.  out[0..7] gate_up, out[8..15] down: cluster size, K slices per expert, grid, output blocks, groups, max groups
+ * per work item, ring stages, shared-memory bytes; out[16] = U_max = min(n_experts, T * top_k); out[17] = the number of
+ * coverage violations over U = 1..U_max (a (expert slot, group) round of a block owned other than exactly once, or rank 0
+ * reading a receive slot no rank wrote in that wave).                                                                  */
+int paro_debug_moe_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out);
 
 /* Debug / test aid: dequantise the prepacked weights back to a dense [K, N] matrix of
  * shape->dtype (the exact operand the GEMM consumes).                                    */

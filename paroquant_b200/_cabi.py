@@ -50,7 +50,17 @@ class ParoChainStep(ctypes.Structure):
     ]
 
 
-ABI_VERSION = 3
+class ParoMoEDesc(ctypes.Structure):
+    """struct paro_moe_desc"""
+
+    _fields_ = [
+        ("gate_up", ctypes.POINTER(ParoLinearShape)), ("down", ctypes.POINTER(ParoLinearShape)), ("n_experts", ctypes.c_int32),
+        ("gate_up_packed", ctypes.c_void_p), ("gate_up_stride", ctypes.c_size_t), ("down_packed", ctypes.c_void_p),
+        ("down_stride", ctypes.c_size_t),
+    ]
+
+
+ABI_VERSION = 4
 CHAIN_MAX_STEPS = 6
 XOP_NONE, XOP_SILU_MUL, XOP_RMSNORM = 0, 1, 2
 EPI_STORE, EPI_ADD_RESIDUAL = 0, 1
@@ -100,6 +110,13 @@ def lib() -> ctypes.CDLL:
         L.paro_debug_gemm_plan.argtypes = [shp, i64, i32, ctypes.POINTER(ctypes.c_int32)]
         L.paro_debug_stream_trace.restype = ctypes.c_int
         L.paro_debug_stream_trace.argtypes = [vp, i32]
+        moe = ctypes.POINTER(ParoMoEDesc)
+        L.paro_moe_workspace_bytes.restype = sz
+        L.paro_moe_workspace_bytes.argtypes = [moe, i64, i32]
+        L.paro_moe_forward.restype = ctypes.c_int
+        L.paro_moe_forward.argtypes = [moe, vp, vp, vp, i64, i32, vp, vp, vp, sz, vp]
+        L.paro_debug_moe_plan.restype = ctypes.c_int
+        L.paro_debug_moe_plan.argtypes = [moe, i64, i32, i32, ctypes.POINTER(ctypes.c_int32)]
         if L.paro_abi_version() != ABI_VERSION:
             raise ImportError("libparo_b200.so ABI version mismatch")
         _lib = L
@@ -110,7 +127,7 @@ EXPORTED_SYMBOLS = (
     "paro_abi_version", "paro_last_error", "paro_last_launch_count", "paro_rotate", "paro_rotate_backward", "paro_packed_bytes",
     "paro_prepack", "paro_workspace_bytes", "paro_linear_forward", "paro_unpack_dense", "paro_debug_trace", "paro_debug_decode_plan",
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
-    "paro_debug_gemm_plan",
+    "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan",
 )
 
 
@@ -223,8 +240,9 @@ def packed_bytes(shape: ParoLinearShape) -> int:
     return n
 
 
-def prepack(shape: ParoLinearShape, qweight, qzeros, scales, pairs, theta, channel_scales) -> torch.Tensor:
-    """AWQ + rotation buffers -> one uint8 tensor in the streaming layout (csrc/paro_layout.h)."""
+def prepack(shape: ParoLinearShape, qweight, qzeros, scales, pairs, theta, channel_scales, out: torch.Tensor | None = None) -> torch.Tensor:
+    """AWQ + rotation buffers -> one uint8 tensor in the streaming layout (csrc/paro_layout.h).  `out`: a caller-owned
+    uint8 buffer of at least packed_bytes(shape) bytes, 128-byte aligned (e.g. one expert's row of a stacked buffer)."""
     dev = _need_cuda(qweight, qzeros, scales, pairs, theta, channel_scales)
     K, N, P, R = shape.in_features, shape.out_features, shape.n_parts, shape.krot
     G = shape.group_size
@@ -236,7 +254,12 @@ def prepack(shape: ParoLinearShape, qweight, qzeros, scales, pairs, theta, chann
             raise RuntimeError(f"prepack: {name} must be {shp} {dt or 'float'}, got {tuple(t.shape)} {t.dtype}")
     qweight, qzeros, scales, pairs, theta = (t.contiguous() for t in (qweight, qzeros, scales, pairs, theta))
     cs = channel_scales.reshape(P, -1).contiguous()
-    packed = torch.empty(packed_bytes(shape), dtype=torch.uint8, device=dev)
+    if out is None:
+        packed = torch.empty(packed_bytes(shape), dtype=torch.uint8, device=dev)
+    else:
+        if out.device != dev or out.dtype != torch.uint8 or not out.is_contiguous() or out.numel() < packed_bytes(shape):
+            raise RuntimeError(f"prepack: out must be a contiguous uint8 tensor of >= {packed_bytes(shape)} bytes on {dev}")
+        packed = out
     with torch.cuda.device(dev):
         rc = lib().paro_prepack(ctypes.byref(shape), qweight.data_ptr(), qzeros.data_ptr(), scales.data_ptr(),
                                 dtype_code(scales.dtype), pairs.data_ptr(), theta.data_ptr(), dtype_code(theta.dtype),
@@ -306,3 +329,43 @@ def chain_forward(steps, n: int, M: int, workspace: torch.Tensor) -> None:
     with torch.cuda.device(dev):
         rc = lib().paro_chain_forward(steps, n, M, workspace.data_ptr(), workspace.numel(), _stream(dev))
     _check(rc, "chain_forward")
+
+
+def moe_workspace_bytes(desc: ParoMoEDesc, T: int, top_k: int) -> int:
+    nb = lib().paro_moe_workspace_bytes(ctypes.byref(desc), T, top_k)
+    if nb == 0:
+        raise RuntimeError(f"moe: {lib().paro_last_error().decode()}")
+    return nb
+
+
+def moe_forward(desc: ParoMoEDesc, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor, h: torch.Tensor, y: torch.Tensor,
+                workspace: torch.Tensor) -> None:
+    """paro_moe_forward on the current stream of x's device: x [T, hidden], topk_ids [T, k] int32, topk_weights [T, k] fp32,
+    h [T, k, 2I] and y [T, hidden] of the experts' dtype, all contiguous on one CUDA device."""
+    dt = _CODE_DTYPE[desc.gate_up.contents.dtype]
+    H, I2 = desc.gate_up.contents.in_features, desc.gate_up.contents.out_features
+    if topk_ids.dtype != torch.int32 or topk_weights.dtype != torch.float32:
+        raise RuntimeError(f"moe_forward: topk_ids must be int32 and topk_weights float32, got {topk_ids.dtype} / {topk_weights.dtype}")
+    for name, t in (("x", x), ("h", h), ("y", y)):
+        if t.dtype != dt:
+            raise RuntimeError(f"moe_forward: {name} must be {dt}, got {t.dtype}")
+    dev = _need_cuda(x, topk_ids, topk_weights, h, y, workspace)
+    if topk_ids.dim() != 2 or tuple(topk_weights.shape) != tuple(topk_ids.shape):
+        raise RuntimeError("moe_forward: topk_ids and topk_weights must both be [T, k]")
+    T, k = topk_ids.shape
+    want = {"x": ((T, H), x), "h": ((T, k, I2), h), "y": ((T, H), y)}
+    for name, (shp, t) in want.items():
+        if tuple(t.shape) != shp:
+            raise RuntimeError(f"moe_forward: {name} must be {shp}, got {tuple(t.shape)}")
+    if not all(t.is_contiguous() for t in (x, topk_ids, topk_weights, h, y)):
+        raise RuntimeError("moe_forward: all tensors must be contiguous")
+    with torch.cuda.device(dev):
+        rc = lib().paro_moe_forward(ctypes.byref(desc), x.data_ptr(), topk_ids.data_ptr(), topk_weights.data_ptr(), T, k, h.data_ptr(),
+                                    y.data_ptr(), workspace.data_ptr(), workspace.numel(), _stream(dev))
+    _check(rc, "moe_forward")
+
+
+def debug_moe_plan(desc: ParoMoEDesc, T: int, top_k: int, sms: int) -> list[int]:
+    out = (ctypes.c_int32 * 18)()
+    _check(lib().paro_debug_moe_plan(ctypes.byref(desc), T, top_k, sms, out), "debug_moe_plan")
+    return list(out)

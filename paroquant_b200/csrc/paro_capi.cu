@@ -51,6 +51,10 @@ size_t gemm_workspace_bytes(const Layout &L, int64_t max_m);
 int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out);
 int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
                  const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);
+int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const float *wts, int64_t T, int32_t k, void *h, void *y,
+                void *workspace, size_t workspace_bytes, cudaStream_t stream);
+int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, int32_t *out);
 
 // rows up to which the persistent small-M kernel serves a linear; above, the rotation pre-pass + GEMM path (knob for A/B runs)
 static int small_m_max() {
@@ -281,6 +285,19 @@ int paro_debug_stream_plan(const paro_linear_shape *shape, int64_t M, int32_t se
   if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_stream_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
   if (!out) { set_error("debug_stream_plan: bad arguments"); return PARO_EINVAL; }
   return stream_debug_plan(L, M, sets, ctas, out);
+}
+
+size_t paro_moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t top_k) { return moe_workspace_bytes(d, T, top_k); }
+
+int paro_moe_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_ids, const float *topk_weights, int64_t T, int32_t top_k,
+                     void *h, void *y, void *workspace, size_t workspace_bytes, paro_stream_t stream) {
+  g_launches = 0;
+  return moe_forward(d, x, topk_ids, topk_weights, T, top_k, h, y, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int paro_debug_moe_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out) {
+  if (!out || sms < 1) { set_error("debug_moe_plan: bad arguments"); return PARO_EINVAL; }
+  return moe_debug_plan(d, T, top_k, sms, out);
 }
 
 int paro_debug_stream_trace(unsigned long long *host_out, int32_t max_ctas) {

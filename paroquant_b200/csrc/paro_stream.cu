@@ -267,12 +267,6 @@ __device__ __forceinline__ void stm_fetch_meta(const StepDesc &S, int part, int 
   }
 }
 
-// silu as vLLM's silu_and_mul computes it: T(x / (1 + exp(-x))) in fp32, then the product in T
-template <typename T> __device__ __forceinline__ uint32_t silu_mul2(uint32_t g2, uint32_t u2) {
-  const float2 g = Traits<T>::to_float2(unpack2<T>(g2));
-  const float a = g.x / (1.0f + __expf(-g.x)), b = g.y / (1.0f + __expf(-g.y));
-  return pack2<T>(__hmul2(Traits<T>::from_floats(a, b), unpack2<T>(u2)));
-}
 // RMSNorm as vLLM's (fused_add_)rms_norm: T(T(h * rstd) * w)
 template <typename T> __device__ __forceinline__ uint32_t norm2(uint32_t h2, float rstd, uint32_t w2) {
   const float2 h = Traits<T>::to_float2(unpack2<T>(h2));

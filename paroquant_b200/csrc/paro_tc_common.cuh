@@ -318,6 +318,14 @@ __device__ __forceinline__ void scale_and_stage(uint32_t rot, int lane, const ui
   }
 }
 
+// silu as vLLM's silu_and_mul computes it: T(x / (1 + exp(-x))) in fp32, then the product in T (paro_stream.cu's SILU_MUL x op
+// and paro_moe.cu's down prologue)
+template <typename T> __device__ __forceinline__ uint32_t silu_mul2(uint32_t g2, uint32_t u2) {
+  const float2 g = Traits<T>::to_float2(unpack2<T>(g2));
+  const float a = g.x / (1.0f + __expf(-g.x)), b = g.y / (1.0f + __expf(-g.y));
+  return pack2<T>(__hmul2(Traits<T>::from_floats(a, b), unpack2<T>(u2)));
+}
+
 template <typename T>
 __device__ __forceinline__ void sincos2(uint32_t theta_pair_bits, float &c0, float &s0, float &c1, float &s1) {
   const float2 th = Traits<T>::to_float2(unpack2<T>(theta_pair_bits));

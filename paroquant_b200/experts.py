@@ -7,13 +7,19 @@ The reference quantises a fused expert block with ONE rotation per projection sh
 down).  Here every expert is two fused linears -- merged gate|up (two partitions carrying the same rotation) and down -- so an
 expert costs two launches, or ONE for decode batches (a two-step chain with SiLU*up folded into the down step).  The rotation is
 recomputed per selected expert inside the kernel (it is a prologue of a few microseconds); routing stays in torch.
+
+`decode_step(T, top_k)` runs the whole block for a decode batch in two launches with the routing read on the device
+(include/paro_b200.h: paro_moe_forward): no host synchronisation, CUDA-graph capturable with the routing changing between replays.
 """
 from __future__ import annotations
 
+import ctypes
+
 import torch
 
+from . import _cabi
 from .chain import ChainStep, ParoChain
-from .checkpoint import ParoLayerBuffers
+from .checkpoint import ParoLayerBuffers, validate_pairs
 from .linear import ParoLinearKernel
 
 
@@ -23,8 +29,38 @@ class ParoExperts:
 
     def __init__(self, blocks: list[dict[str, ParoLayerBuffers]], dtype: torch.dtype = torch.bfloat16, device="cuda", check_pairs: bool = False):
         self.dtype = dtype
-        self.gate_up = [ParoLinearKernel.from_buffers(b["gate_up"].to(device), dtype, check_pairs=check_pairs) for b in blocks]
-        self.down = [ParoLinearKernel.from_buffers(b["down"].to(device), dtype, check_pairs=check_pairs) for b in blocks]
+        self.n_experts = len(blocks)
+        if self.n_experts < 1:
+            raise RuntimeError("ParoExperts needs at least one expert")
+        # the decode kernels (decode_step) read one rotation per projection: every expert must carry the same one, and gate and up
+        # the same as each other (convert.py:281-381 stores it once per block)
+        for proj in ("gate_up", "down"):
+            r0 = blocks[0][proj]
+            for e, b in enumerate(blocks):
+                r = b[proj]
+                if not all(torch.equal(getattr(r, n).cpu(), getattr(r0, n).cpu()) for n in ("theta", "pairs", "channel_scales")):
+                    raise RuntimeError(f"expert {e}: its {proj} rotation differs from expert 0's; an expert block shares one rotation per projection")
+        gu0 = blocks[0]["gate_up"]
+        if not all(torch.equal(getattr(gu0, n)[0].cpu(), getattr(gu0, n)[1].cpu()) for n in ("theta", "pairs", "channel_scales")):
+            raise RuntimeError("gate and up carry different rotations; an expert block's merged gate_up shares one")
+        # every expert prepacked into ONE stacked buffer per projection, [E, stride]; the per-expert kernels wrap row views of it
+        self.gate_up, self.down = [], []
+        self.packed, self.shapes, self.strides = {}, {}, {}
+        for proj, kernels in (("gate_up", self.gate_up), ("down", self.down)):
+            b0 = blocks[0][proj]
+            shape = _cabi.make_shape(b0.qweight.shape[0], b0.part_sizes, b0.group_size, b0.theta.shape[-2], dtype)
+            stride = (_cabi.packed_bytes(shape) + 255) // 256 * 256
+            stack = torch.empty(self.n_experts, stride, dtype=torch.uint8, device=device)
+            for e, b in enumerate(blocks):
+                b = b[proj].to(device)
+                theta, pairs, cs = b.theta, b.pairs, b.channel_scales
+                if theta.dim() == 2:
+                    theta, pairs, cs = theta[None], pairs[None], cs.reshape(1, -1)
+                if check_pairs:
+                    validate_pairs(pairs, b.group_size)
+                _cabi.prepack(shape, b.qweight, b.qzeros, b.scales, pairs, theta, cs, out=stack[e])
+                kernels.append(ParoLinearKernel(stack[e], shape))
+            self.packed[proj], self.shapes[proj], self.strides[proj] = stack, shape, stride
         self.hidden = self.down[0].shape.out_features
         self.inter = self.down[0].shape.in_features
         self._chains: dict[tuple[int, int], tuple] = {}
@@ -60,3 +96,43 @@ class ParoExperts:
             y = self.expert_forward(int(e), x[rows].contiguous())
             out.index_add_(0, rows, y.float() * topk_weights[rows, slot].float()[:, None])
         return out.to(x.dtype)
+
+    def desc(self) -> _cabi.ParoMoEDesc:
+        """The C descriptor of the stacked expert buffers (kept alive by this object)."""
+        d = _cabi.ParoMoEDesc()
+        d.gate_up, d.down = ctypes.pointer(self.shapes["gate_up"]), ctypes.pointer(self.shapes["down"])
+        d.n_experts = self.n_experts
+        d.gate_up_packed, d.gate_up_stride = self.packed["gate_up"].data_ptr(), self.strides["gate_up"]
+        d.down_packed, d.down_stride = self.packed["down"].data_ptr(), self.strides["down"]
+        return d
+
+    def decode_step(self, T: int, top_k: int) -> "ParoMoEStep":
+        """The block for T <= 16 tokens with top_k slots each over fixed device buffers (see ParoMoEStep)."""
+        return ParoMoEStep(self, T, top_k)
+
+
+class ParoMoEStep:
+    """The expert block of one decode step over fixed device buffers, like ParoChain: write the inputs into `x` [T, hidden],
+    `topk_ids` [T, k] int32 and `topk_weights` [T, k] fp32 (int64 ids from torch.topk convert with a device `copy_`), call
+    `step()`, read `y` [T, hidden].  `h` [T, k, 2I] holds every valid slot's gate|up output.  Construction allocates; a call
+    never does, never synchronises the host, and launches two kernels on the current stream, so it can be captured in a CUDA
+    graph whose replays see whatever routing the buffers hold."""
+
+    def __init__(self, experts: ParoExperts, T: int, top_k: int):
+        dev = experts.packed["gate_up"].device
+        self.experts, self.T, self.top_k = experts, int(T), int(top_k)
+        self._desc = experts.desc()
+        nbytes = _cabi.moe_workspace_bytes(self._desc, self.T, self.top_k)
+        dt = experts.dtype
+        self.x = torch.zeros(self.T, experts.hidden, dtype=dt, device=dev)
+        self.topk_ids = torch.zeros(self.T, self.top_k, dtype=torch.int32, device=dev)
+        self.topk_weights = torch.zeros(self.T, self.top_k, dtype=torch.float32, device=dev)
+        self.h = torch.zeros(self.T, self.top_k, 2 * experts.inter, dtype=dt, device=dev)
+        self.y = torch.zeros(self.T, experts.hidden, dtype=dt, device=dev)
+        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+
+    def step(self) -> torch.Tensor:
+        _cabi.moe_forward(self._desc, self.x, self.topk_ids, self.topk_weights, self.h, self.y, self.workspace)
+        return self.y
+
+    __call__ = step
