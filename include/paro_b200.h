@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define PARO_ABI_VERSION 4
+#define PARO_ABI_VERSION 5
 #define PARO_MAX_PARTS 8
 
 /* element types (activations, rotation parameters, scales) */
@@ -237,6 +237,12 @@ int paro_debug_moe_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_
  * shape->dtype (the exact operand the GEMM consumes).                                    */
 int paro_unpack_dense(const paro_linear_shape *shape, const void *packed, void *W_out,
                       paro_stream_t stream);
+
+/* Debug / test aid: act[m, i] = T(T(silu(gate[m, i])) * up[m, i]) for device gate_up [M, 2I] (gate | up) and act [M, I]
+ * of dtype (PARO_F16 | PARO_BF16), both 4-byte aligned, I even.  The library's own SiLU * up, bit-identical to the
+ * operand paro_moe_forward's down launch and the chains' PARO_XOP_SILU_MUL step rotate (its exp is the fast one, which
+ * an fp32 or fp64 exp does not reproduce bit for bit).                                                                */
+int paro_debug_silu_mul(int32_t dtype, const void *gate_up, void *act, int64_t M, int32_t I, paro_stream_t stream);
 
 /* Number of kernels the last successful paro_linear_forward / paro_rotate call on this
  * thread launched (bench.py's gpu_launches accounting).                                  */

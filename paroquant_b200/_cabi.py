@@ -60,7 +60,7 @@ class ParoMoEDesc(ctypes.Structure):
     ]
 
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 CHAIN_MAX_STEPS = 6
 XOP_NONE, XOP_SILU_MUL, XOP_RMSNORM = 0, 1, 2
 EPI_STORE, EPI_ADD_RESIDUAL = 0, 1
@@ -96,6 +96,8 @@ def lib() -> ctypes.CDLL:
         L.paro_linear_forward.argtypes = [shp, vp, vp, i64, vp, vp, vp, sz, vp]
         L.paro_unpack_dense.restype = ctypes.c_int
         L.paro_unpack_dense.argtypes = [shp, vp, vp, vp]
+        L.paro_debug_silu_mul.restype = ctypes.c_int
+        L.paro_debug_silu_mul.argtypes = [i32, vp, vp, i64, i32, vp]
         L.paro_debug_trace.restype = ctypes.c_int
         L.paro_debug_trace.argtypes = [vp, i32]
         L.paro_chain_workspace_bytes.restype = sz
@@ -127,7 +129,7 @@ EXPORTED_SYMBOLS = (
     "paro_abi_version", "paro_last_error", "paro_last_launch_count", "paro_rotate", "paro_rotate_backward", "paro_packed_bytes",
     "paro_prepack", "paro_workspace_bytes", "paro_linear_forward", "paro_unpack_dense", "paro_debug_trace", "paro_debug_decode_plan",
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
-    "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan",
+    "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan", "paro_debug_silu_mul",
 )
 
 
@@ -310,6 +312,24 @@ def unpack_dense(shape: ParoLinearShape, packed: torch.Tensor) -> torch.Tensor:
         rc = lib().paro_unpack_dense(ctypes.byref(shape), packed.data_ptr(), W.data_ptr(), _stream(dev))
     _check(rc, "unpack_dense")
     return W
+
+
+def debug_silu_mul(gate_up: torch.Tensor) -> torch.Tensor:
+    """gate_up [..., 2I] (gate | up) -> [..., I]: the library's SiLU * up, bit-identical to the operand the MoE down launch
+    and a chain's silu_mul step rotate (tests)."""
+    if gate_up.dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError(f"debug_silu_mul: gate_up must be float16 or bfloat16, got {gate_up.dtype}")
+    if gate_up.dim() < 1 or gate_up.size(-1) < 4 or gate_up.size(-1) % 4:
+        raise RuntimeError(f"debug_silu_mul: the last dimension must be 2I with I even and >= 2, got {tuple(gate_up.shape)}")
+    dev = _need_cuda(gate_up)
+    gate_up = gate_up.contiguous()
+    I = gate_up.size(-1) // 2
+    act = torch.empty(*gate_up.shape[:-1], I, dtype=gate_up.dtype, device=dev)
+    with torch.cuda.device(dev):
+        rc = lib().paro_debug_silu_mul(dtype_code(gate_up.dtype), gate_up.data_ptr(), act.data_ptr(), act.numel() // max(I, 1), I,
+                                       _stream(dev))
+    _check(rc, "debug_silu_mul")
+    return act
 
 
 def last_launch_count() -> int:

@@ -55,6 +55,7 @@ size_t moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);
 int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const float *wts, int64_t T, int32_t k, void *h, void *y,
                 void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, int32_t *out);
+int moe_debug_silu_mul(int dtype, const void *gate_up, void *act, int64_t M, int I, cudaStream_t stream);
 
 // rows up to which the persistent small-M kernel serves a linear; above, the rotation pre-pass + GEMM path (knob for A/B runs)
 static int small_m_max() {
@@ -196,6 +197,15 @@ int paro_unpack_dense(const paro_linear_shape *shape, const void *packed, void *
   if (!shape || !make_layout(*shape, L, &why)) { set_error("unpack_dense: %s", shape ? why : "null shape"); return PARO_EINVAL; }
   if (!packed || !W_out) { set_error("unpack_dense: null pointer argument"); return PARO_EINVAL; }
   return unpack_dense_launch(*shape, L, packed, W_out, static_cast<cudaStream_t>(stream));
+}
+
+int paro_debug_silu_mul(int32_t dtype, const void *gate_up, void *act, int64_t M, int32_t I, paro_stream_t stream) {
+  g_launches = 0;
+  if (dtype != PARO_F16 && dtype != PARO_BF16) { set_error("debug_silu_mul: dtype must be F16 or BF16, got code %d", dtype); return PARO_EINVAL; }
+  if (M < 0 || I < 2 || I % 2) { set_error("debug_silu_mul: M >= 0 and an even I >= 2 needed, got M = %lld, I = %d", static_cast<long long>(M), I); return PARO_EINVAL; }
+  if (!gate_up || !act) { set_error("debug_silu_mul: null pointer argument"); return PARO_EINVAL; }
+  if (!aligned(gate_up, 4) || !aligned(act, 4)) { set_error("debug_silu_mul: gate_up / act must be 4-byte aligned"); return PARO_EINVAL; }
+  return moe_debug_silu_mul(dtype, gate_up, act, M, I, static_cast<cudaStream_t>(stream));
 }
 
 int paro_debug_decode_plan(const paro_linear_shape *shape, int64_t M, int32_t sets, int32_t sms, const int32_t *resident_clusters,

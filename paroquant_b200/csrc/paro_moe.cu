@@ -552,4 +552,29 @@ int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, in
   return PARO_OK;
 }
 
+// Test hook: act[m, i] = silu_mul2(gate[m, i], up[m, i]) -- the down launch's operand before its rotation, from the same
+// device function compiled with the same flags, so tests can rebuild it bit for bit.  One thread per element pair.
+template <typename T>
+__global__ void silu_mul_kernel(const uint32_t *__restrict__ gu, uint32_t *__restrict__ act, int64_t M, int I2) {
+  const int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (idx >= M * I2) return;
+  const int64_t m = idx / I2;
+  const int j = static_cast<int>(idx - m * I2);
+  act[idx] = silu_mul2<T>(gu[m * 2 * I2 + j], gu[m * 2 * I2 + I2 + j]);
+}
+
+int moe_debug_silu_mul(int dtype, const void *gate_up, void *act, int64_t M, int I, cudaStream_t stream) {
+  if (M == 0) return PARO_OK;
+  const int I2 = I / 2;
+  const int B = 256;
+  const unsigned grid = static_cast<unsigned>((M * I2 + B - 1) / B);
+  const uint32_t *gu = static_cast<const uint32_t *>(gate_up);
+  uint32_t *out = static_cast<uint32_t *>(act);
+  if (dtype == PARO_BF16) silu_mul_kernel<__nv_bfloat16><<<grid, B, 0, stream>>>(gu, out, M, I2);
+  else silu_mul_kernel<__half><<<grid, B, 0, stream>>>(gu, out, M, I2);
+  PARO_CUDA_OK(cudaGetLastError());
+  note_launches(1);
+  return PARO_OK;
+}
+
 }  // namespace paro

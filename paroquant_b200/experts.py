@@ -89,9 +89,11 @@ class ParoExperts:
         return self.down[e](torch.nn.functional.silu(gu[:, : self.inter]) * gu[:, self.inter:])
 
     def __call__(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor) -> torch.Tensor:
-        """x [T, hidden], topk_ids / topk_weights [T, k] -> sum_k w_k * expert_{id_k}(x) in fp32, rounded once."""
+        """x [T, hidden], topk_ids / topk_weights [T, k] -> sum_k w_k * expert_{id_k}(x) in fp32, rounded once.  A slot whose id
+        lies outside [0, n_experts) contributes nothing, as in decode_step (expert parallelism marks non-local experts with -1)."""
         out = torch.zeros(x.shape[0], self.hidden, dtype=torch.float32, device=x.device)
-        for e in torch.unique(topk_ids).tolist():
+        valid = (topk_ids >= 0) & (topk_ids < self.n_experts)
+        for e in torch.unique(topk_ids[valid]).tolist():
             rows, slot = (topk_ids == e).nonzero(as_tuple=True)
             y = self.expert_forward(int(e), x[rows].contiguous())
             out.index_add_(0, rows, y.float() * topk_weights[rows, slot].float()[:, None])

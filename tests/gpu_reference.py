@@ -76,3 +76,78 @@ def check_linear(k, L, x: torch.Tensor, y: torch.Tensor, bias: torch.Tensor | No
     """`check` for the output y of ParoLinearKernel k (layer buffers L on the GPU) on input x: the reference rotates x with the
     standalone rotate kernel and multiplies with k's own dequantised operand (pass W to reuse one)."""
     return check(y, rotated(L, x), k.dense_weight() if W is None else W, L.part_sizes, bias, what)
+
+
+COMBINE_REL = 2.0 ** -24
+
+
+def check_combine(y: torch.Tensor, tok: torch.Tensor, w: torch.Tensor, ys: torch.Tensor, mag: torch.Tensor, what: str = "",
+                  show: int = 6) -> float:
+    """Element-wise check of a MoE block's output y [T, N] in T (include/paro_b200.h: paro_moe_forward).  One entry j per valid
+    slot (a duplicate id is one entry per occurrence): tok[j] its token, w[j] its weight, ys[j] [N] the exact fp64 expert output
+    sum_k xr[k] * W[k, n] and mag[j] [N] = sum_k |xr[k] * W[k, n]|.  The block computes v_j = T(fp32 sum, any order),
+    p_j = fp32(v_j * w_j) and out[t] = T(fp32 sum of p_j from 0, any order).  With ref[t] = T(sum_j w_j ys[j]) in fp64:
+
+      |v_j - ys_j|   <= ulp_T(T(ys_j)) + 2^-16 mag_j         (rounding of the fp32 sum to T, a flip at a binade edge included,
+                                                              plus `check`'s bound on the fp32 sum)
+      |S - sum w v|  <= n 2^-24 sum_j |w_j v_j|              (n fp32 roundings: n products, n - 1 adds; first order)
+      |T(S) - ref|   <= ulp_T(ref) + |S - sum_j w_j ys_j|    (the two roundings to T, a tie flip included)
+
+    so every element of a token with n valid slots must satisfy
+
+      |out - ref| <= ulp_T(ref) + sum_j |w_j| (ulp_T(T(ys_j)) + 2^-16 mag_j) + (n + 1) 2^-24 sum_j |w_j ys_j|
+
+    where the + 1 covers |v_j| > |ys_j| and the second-order terms.  A token with no valid slot must be exactly 0.  Raises
+    AssertionError naming the violating elements as (token, column, 128-column block) with got / ref / tol; returns the
+    largest err / tol."""
+    dt = y.dtype
+    T, N = y.shape
+    dev = ys.device
+    tok, wd = tok.to(dev).long(), w.to(dev).double()
+    ys, mag = ys.double(), mag.double()
+    z = lambda: torch.zeros(T, N, dtype=torch.float64, device=dev)
+    exact = z().index_add_(0, tok, wd[:, None] * ys)
+    slot_tol = z().index_add_(0, tok, wd.abs()[:, None] * (ulp(ys.to(dt), dt) + SUM_REL * mag))
+    absum = z().index_add_(0, tok, (wd[:, None] * ys).abs())
+    n = torch.bincount(tok, minlength=T).double()[:, None]
+    ref = exact.to(dt)
+    tol = ulp(ref, dt) + slot_tol + (n + 1) * COMBINE_REL * absum
+    y2 = y.to(dev)
+    err = (y2.double() - ref.double()).abs()
+    empty = (n == 0).expand(T, N)
+    bad = torch.where(empty, y2.double() != 0, ~(err <= tol))   # NaN / inf count as violations
+    if bool(bad.any()):
+        idx = bad.nonzero().tolist()
+        lines = [f"  (token {t}, col {c}, block {c // 128}): got {float(y2[t, c]):.6g} ref {float(ref[t, c]):.6g} "
+                 f"tol {'0 (no valid slot)' if bool(empty[t, c]) else format(float(tol[t, c]), '.3g')}" for t, c in idx[:show]]
+        raise AssertionError(f"{what}: {len(idx)} of {bad.numel()} elements outside the element-wise bound\n" + "\n".join(lines))
+    full = ~empty
+    return float((err[full] / tol[full]).max()) if bool(full.any()) else 0.0
+
+
+def check_moe(y: torch.Tensor, h: torch.Tensor, ids: torch.Tensor, w: torch.Tensor, experts, down, what: str = "") -> float:
+    """`check_combine` for the output y [T, N] of a MoE block (ParoExperts `experts`, down rotation buffers `down`) from the
+    block's own gate|up output h [T, k, 2I]: for every valid slot (t, s), act = the library's SiLU * up of h[t, s] (bit-identical
+    to the down launch's operand), xr = act rotated by the standalone rotate kernel, ys = xr . W_d[e] in fp64 with W_d[e]
+    expert e's dequantised down operand.  Ids outside [0, E) are dropped.  With `check` on h per expert, both launches are
+    checked element-wise."""
+    from paroquant_b200 import _cabi
+    dev = h.device
+    ids, w = ids.to(dev).long(), w.to(dev).float()
+    Ld = down.to(dev)
+    tok, ws, ys, mag = [], [], [], []
+    valid = (ids >= 0) & (ids < experts.n_experts)
+    for e in torch.unique(ids[valid]).tolist():
+        rows, slot = (ids == e).nonzero(as_tuple=True)
+        xr = rotated(Ld, _cabi.debug_silu_mul(h[rows, slot]))[0].double()
+        Wd = experts.down[e].dense_weight().double()
+        ys.append(xr @ Wd)
+        mag.append(xr.abs() @ Wd.abs())
+        tok.append(rows)
+        ws.append(w[rows, slot])
+        del Wd
+    N = y.shape[1]
+    if not tok:
+        tok, ws = [torch.zeros(0, dtype=torch.long, device=dev)], [torch.zeros(0, device=dev)]
+        ys = mag = [torch.zeros(0, N, dtype=torch.float64, device=dev)]
+    return check_combine(y, torch.cat(tok), torch.cat(ws), torch.cat(ys), torch.cat(mag), what)

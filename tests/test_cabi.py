@@ -25,7 +25,27 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/paro_b200.h but not exported"
     assert set(names) == set(_cabi.EXPORTED_SYMBOLS)
-    assert lib.paro_abi_version() == _cabi.ABI_VERSION
+    assert lib.paro_abi_version() == _cabi.ABI_VERSION == 5
+
+
+def test_debug_silu_mul_argument_checks():
+    """paro_debug_silu_mul's host-side checks (no launch): dtype, an even I, pointers and alignment; no rows is a no-op."""
+    lib = _cabi.lib()
+    buf = (ctypes.c_char * 4096)()
+    p = (ctypes.addressof(buf) + 255) // 256 * 256
+    for args, code, msg in (((0, p, p, 1, 8), 1, b"F16 or BF16"), ((2, p, p, 1, 7), 1, b"even I"), ((2, p, p, -1, 8), 1, b"M >= 0"),
+                            ((2, None, p, 1, 8), 1, b"null pointer"), ((1, p + 2, p, 1, 8), 1, b"4-byte aligned"),
+                            ((2, p, p, 0, 8), 0, None)):
+        rc = lib.paro_debug_silu_mul(*args, None)
+        assert rc == code and (msg is None or msg in lib.paro_last_error()), (args, rc, lib.paro_last_error())
+    assert lib.paro_last_launch_count() == 0
+    with pytest.raises(RuntimeError, match="CUDA-only"):
+        _cabi.debug_silu_mul(torch.zeros(2, 16, dtype=torch.bfloat16))
+    for last in (17, 18, 2):   # gate | up halves must each have an even width: an odd last dimension would shift the up half
+        with pytest.raises(RuntimeError, match="last dimension must be 2I"):
+            _cabi.debug_silu_mul(torch.zeros(2, last, dtype=torch.bfloat16))
+    with pytest.raises(RuntimeError, match="float16 or bfloat16"):
+        _cabi.debug_silu_mul(torch.zeros(2, 16))
 
 
 def test_struct_layout_matches_header():

@@ -1,13 +1,16 @@
 """The MoE expert block in two launches with device-side routing (ParoExperts.decode_step, include/paro_b200.h:
-paro_moe_forward) against the oracle composed per expert (oracle.linear / oracle.silu_and_mul, fp64 combine), stage-wise
-against the standalone rotate kernel and each expert's dequantised operand, over routing edge cases, for bit invariance, under
-CUDA-graph replay with changing routings, and with no host work.  Reference semantics: mlx/modules.py:159-212 (RotateSwitchGLU)
-on the format of convert.py:281-406."""
+paro_moe_forward) against the oracle composed per expert (oracle.linear / oracle.silu_and_mul, fp64 combine), element-wise
+against fp64 (h against the standalone rotate kernel and each expert's dequantised operand, y against the library's own SiLU *
+up of that h, rotated, times each expert's dense down operand; tests/gpu_reference.py) over a table of shapes whose launch
+plans cover the planner's features (tests/moe_cases.py), over routing edge cases, for bit invariance, under CUDA-graph replay
+with changing routings, and with no host work.  Reference semantics: mlx/modules.py:159-212 (RotateSwitchGLU) on the format of
+convert.py:281-406."""
 import numpy as np
 import pytest
 import torch
 
-from gpu_reference import check
+from gpu_reference import check, check_moe, rotated, ulp
+from moe_cases import CASES, ROUTINGS, routing
 from paroquant_b200.checkpoint import ParoLayerBuffers, make_synthetic_activations, make_synthetic_layer
 
 pytestmark = pytest.mark.gpu
@@ -15,13 +18,13 @@ TOL = 2e-3       # two fused linears and an activation deep (the existing expert
 ROW_TOL = 1.5e-2  # one token's row: a few bf16 roundings (2^-8 each) deep; a missing expert moves a row by tens of percent
 
 
-def _blocks(E, H, I, group=128, krot=8):
-    shared_gu = make_synthetic_layer(H, [I, I], group_size=group, krot=krot, seed=70)
-    shared_d = make_synthetic_layer(I, [H], group_size=group, krot=krot, seed=71)
+def _blocks(E, H, I, group=128, krot=8, device="cpu"):
+    shared_gu = make_synthetic_layer(H, [I, I], group_size=group, krot=krot, seed=70, device=device)
+    shared_d = make_synthetic_layer(I, [H], group_size=group, krot=krot, seed=71, device=device)
     blocks = []
     for e in range(E):
-        gu = make_synthetic_layer(H, [I, I], group_size=group, krot=krot, seed=80 + e)
-        d = make_synthetic_layer(I, [H], group_size=group, krot=krot, seed=90 + e)
+        gu = make_synthetic_layer(H, [I, I], group_size=group, krot=krot, seed=80 + e, device=device)
+        d = make_synthetic_layer(I, [H], group_size=group, krot=krot, seed=90 + e, device=device)
         gu = ParoLayerBuffers(gu.qweight, gu.qzeros, gu.scales, shared_gu.theta.clone(), shared_gu.pairs.clone(), shared_gu.channel_scales.clone(),
                               [I, I], group, None)
         gu.theta[1], gu.pairs[1], gu.channel_scales[1] = gu.theta[0], gu.pairs[0], gu.channel_scales[0]
@@ -122,16 +125,14 @@ def test_moe_qwen3_shaped_block(oracle, T):
 
 
 @pytest.mark.parametrize("T,k", [(1, 2), (6, 8), (16, 4)])
-def test_moe_stagewise(oracle, T, k):
-    """Every valid h[t, s] element-wise against the rotate kernel and the expert's dense operand; out per row against the
-    oracle's silu*mul -> rotate -> down -> combine applied to the GPU's own h."""
-    from gpu_reference import rotated
+def test_moe_stagewise(T, k):
+    """Every valid h[t, s] element-wise against the rotate kernel and the expert's dense operand; y element-wise against the
+    library's SiLU * up of the GPU's own h, rotated, times each expert's dense down operand in fp64, combined in fp64."""
     E, H, I = 8, 256, 384
     blocks, ex = _experts(E, H, I)
     x = make_synthetic_activations(T, H, seed=21 + T, dtype=torch.bfloat16)
     ids, w = _routing(T, k, E, seed=T * k)
     st = _run(ex, x, ids, w)
-    h = st.h.cpu()
     xc = x.cuda()
     for e in range(E):
         rows, slot = (ids.long() == e).nonzero(as_tuple=True)
@@ -140,19 +141,7 @@ def test_moe_stagewise(oracle, T, k):
         L = blocks[e]["gate_up"].to("cuda")
         xr = [r[rows.cuda()] for r in rotated(L, xc)]
         check(st.h[rows.cuda(), slot.cuda()], xr, ex.gate_up[e].dense_weight(), L.part_sizes, what=f"h of expert {e}")
-    ref = np.zeros((T, H), np.float64)
-    for e in range(E):
-        rows, slot = (ids.long() == e).nonzero(as_tuple=True)
-        if not len(rows):
-            continue
-        act = oracle.silu_and_mul(h[rows, slot].float().numpy(), "bfloat16")
-        ye = oracle.linear(act, blocks[e]["down"].numpy_dict(), "bfloat16")
-        np.add.at(ref, rows.numpy(), ye.astype(np.float64) * w[rows, slot].numpy()[:, None].astype(np.float64))
-    ref = oracle.round_to(ref.astype(np.float32), "bfloat16")
-    got = st.y.float().cpu().numpy()
-    assert oracle.rel_err(got, ref) < 1e-3
-    for t in range(T):   # per row: the kernel's SiLU is the fast-math one of the chain kernel, so a row may carry a few flips
-        assert oracle.rel_err(got[t], ref[t]) < 2e-3, f"token {t}"
+    check_moe(st.y, st.h, ids, w, ex, blocks[0]["down"], what="y")
 
 
 def _edge_routings(T, k, E):
@@ -279,3 +268,87 @@ def test_moe_from_disk_checkpoint(oracle, tmp_path):
     bad[2]["down"] = ParoLayerBuffers(d.qweight, d.qzeros, d.scales, d.theta + 0.5, d.pairs, d.channel_scales, d.part_sizes, d.group_size, None)
     with pytest.raises(RuntimeError, match="rotation differs"):
         ParoExperts(bad, torch.bfloat16)
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_debug_silu_mul_within_one_ulp_of_fp64_silu(dtype):
+    """The test hook's SiLU * up (the library's own, with its fast exp): every element is T(s * u) with s within one ulp of
+    T(silu(g)) computed in fp64, and the product rounded once to T; nearly all elements take s = T(silu(g)) itself.  (A one-ulp
+    step of s can move the product by more than one ulp of the product, so the ulp is counted on s.)"""
+    from paroquant_b200 import _cabi
+    g = torch.Generator(device="cuda").manual_seed(0)
+    gu = (torch.randn(48, 2 * 1024, generator=g, device="cuda") * 4).to(dtype)
+    gu[0, :8] = torch.tensor([0.0, -0.0, 1e-3, -1e-3, 30.0, -30.0, 80.0, -80.0], dtype=dtype)
+    act = _cabi.debug_silu_mul(gu)
+    assert _cabi.last_launch_count() == 1
+    gd, ud = gu[:, :1024].double(), gu[:, 1024:].double()
+    s0 = (gd / (1.0 + torch.exp(-gd))).to(dtype).double()
+    du = ulp(s0, dtype)
+    hits = [act.double() == (c.to(dtype).double() * ud).to(dtype).double() for c in (s0, s0 - du, s0 - du / 2, s0 + du)]
+    ok = hits[0] | hits[1] | hits[2] | hits[3]
+    assert bool(ok.all()), f"{int((~ok).sum())} elements are not T(s * u) with s within one ulp of T(silu(g))"
+    assert float(hits[0].double().mean()) > 0.99
+    assert torch.equal(_cabi.debug_silu_mul(gu[5:9]), act[5:9])
+
+
+_case_cache = {}
+
+
+def _case_experts(case):
+    """Weights generated on the device, one shape kept at a time (a Mixtral-shaped block is about 1.5 GB with its buffers)."""
+    from paroquant_b200.experts import ParoExperts
+    key = (case.H, case.I, case.E, case.dtype, case.group, case.krot)
+    if key not in _case_cache:
+        _case_cache.clear()
+        torch.cuda.empty_cache()
+        blocks = _blocks(case.E, case.H, case.I, case.group, case.krot, device="cuda")
+        _case_cache[key] = (blocks, ParoExperts(blocks, case.dtype))
+    return _case_cache[key]
+
+
+def _plan_str(out, U):
+    s = []
+    for name, base in (("gate_up", 0), ("down", 8)):
+        c, S, grid, nb, G, ng, nst, smem = out[base: base + 8]
+        s.append(f"{name} c={c} S={S} waves={-(-U * S // c)} groups/item={ng} stages={nst}")
+    return ", ".join(s)
+
+
+@pytest.mark.parametrize("kind", ROUTINGS)
+@pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
+def test_moe_plan_space_elementwise(case, kind):
+    """Every case of tests/moe_cases.py (together their plans at 132 SMs reach every cluster size, uneven and wave-crossing K
+    slices, reused receive buffers, partial last waves and items longer than the ring) under four routings: h of every selected
+    expert with `check`, y with `check_moe`, every output element written, and a second launch bit-identical."""
+    from paroquant_b200 import _cabi
+    blocks, ex = _case_experts(case)
+    T, k = case.T, case.k
+    x = make_synthetic_activations(T, case.H, seed=17 + T, dtype=case.dtype, device="cuda")
+    ids, w = routing(case, kind)
+    idc = ids.cuda()
+    valid = (idc >= 0) & (idc < case.E)
+    st = ex.decode_step(T, k)
+    st.x.copy_(x)
+    st.topk_ids.copy_(idc)
+    st.topk_weights.copy_(w.cuda())
+    outs = []
+    for _ in range(2):
+        st.h.fill_(float("nan"))
+        st.y.fill_(float("nan"))   # every element of y and of the valid rows of h must be written
+        st.step()
+        outs.append((st.y.clone(), st.h[valid].clone()))
+    assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1]), "a second launch differs"
+
+    Lgu = blocks[0]["gate_up"]
+    xr = rotated(Lgu, x)
+    worst_h = 0.0
+    for e in torch.unique(idc[valid]).tolist():
+        rows, slot = (idc == e).nonzero(as_tuple=True)
+        worst_h = max(worst_h, check(st.h[rows, slot], [r[rows] for r in xr], ex.gate_up[e].dense_weight(), Lgu.part_sizes,
+                                     what=f"{case.name} {kind}: h of expert {e}"))
+    worst_y = check_moe(st.y, st.h, idc, w, ex, blocks[0]["down"], what=f"{case.name} {kind}: y")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    out = _cabi.debug_moe_plan(st._desc, T, k, sms)
+    U = len(torch.unique(idc[valid]))
+    print(f"\n[moe-case] {case.name} {kind}: U={U} of {out[16]}, {sms} SMs: {_plan_str(out, out[16])}; "
+          f"max err/tol h {worst_h:.3f} y {worst_y:.3f}")

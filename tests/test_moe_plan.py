@@ -49,6 +49,37 @@ def test_plan_keeps_both_reference_shapes_busy():
     assert m[2] >= 132 and m[10] >= 64
 
 
+def test_gpu_case_table_reaches_every_plan_feature():
+    """The default plans at 132 SMs of the cases tests/test_gpu_moe.py runs (tests/moe_cases.py) cover every cluster size on
+    each launch and the plan features where the kernel's cross-CTA reduction can go wrong; if the planner drifts away from
+    one, this fails without a GPU."""
+    from moe_cases import CASES
+    cs = {0: set(), 8: set()}
+    seen = set()
+    for case in CASES:
+        out = _cabi.debug_moe_plan(_desc(case.H, case.I, case.E, dtype=case.dtype, group=case.group, krot=case.krot), case.T, case.k, 132)
+        assert out[17] == 0, f"{case.name}: {out[17]} coverage violations"
+        U = out[16]
+        for base in (0, 8):
+            c, S, grid, nb, G, ng_max, nst, smem = out[base: base + 8]
+            cs[base].add(c)
+            waves = -(-U * S // c)
+            if S > 1 and G % S:
+                seen.add("uneven K slices")
+            if any((u * S) // c != (u * S + S - 1) // c for u in range(U)):
+                seen.add("an expert's slices split across a wave boundary")
+            if waves >= 3:
+                seen.add("three or more waves: both receive buffers reused")
+            if (U * S) % c:
+                seen.add("a partial last wave")
+            if ng_max > nst:
+                seen.add("a work item longer than the weight ring")
+    assert cs[0] == {1, 2, 4, 8}, f"gate_up cluster sizes {sorted(cs[0])}"
+    assert cs[8] == {1, 2, 4, 8}, f"down cluster sizes {sorted(cs[8])}"
+    assert seen == {"uneven K slices", "an expert's slices split across a wave boundary", "three or more waves: both receive buffers reused",
+                    "a partial last wave", "a work item longer than the weight ring"}, sorted(seen)
+
+
 def _rc(fn, *args):
     rc = fn(*args)
     return rc, _cabi.lib().paro_last_error().decode()

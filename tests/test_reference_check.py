@@ -1,9 +1,12 @@
-"""The element-wise bound of tests/gpu_reference.py, on the CPU: it accepts any fp32 summation order, and it flags a single
-element that normwise relative error 1e-3 lets through (a 64-channel partial sum missing, or 3 ulps off)."""
+"""The element-wise bounds of tests/gpu_reference.py, on the CPU.  `check` (a fused linear) accepts any fp32 summation order and
+flags a single element that normwise relative error 1e-3 lets through (a 64-channel partial sum missing, or 3 ulps off).
+`check_combine` (a MoE block's weighted sum of expert outputs) accepts any fp32 order of the expert sums and of the slot
+combine, and flags faults of the block's reduction and combine that the oracle comparisons' normwise and per-row bounds let
+through."""
 import pytest
 import torch
 
-from gpu_reference import check, ulp
+from gpu_reference import check, check_combine, ulp
 
 M, K, PARTS = 32, 4096, [1024, 1024]
 
@@ -90,3 +93,141 @@ def test_flags_non_finite_output():
     y[0, 0] = float("nan")
     with pytest.raises(AssertionError, match="1 of 65536"):
         check(y, xrs, W, PARTS)
+
+
+# ---- the MoE combine bound (check_combine): T tokens x k slots of E experts, each slot's rotated row xr [K] against its
+# expert's operand W[e] [K, N]; the block rounds every slot's fp32 sum to T and adds the weighted slots in fp32
+MT, MK, ME, MKK, MN = 4, 4, 4, 2048, 1024
+
+
+def _moe(dt, seed, ids=None, w=None):
+    g = torch.Generator().manual_seed(seed)
+    W = []
+    for _ in range(ME):
+        q = torch.randint(0, 16, (MKK, MN), generator=g) - torch.randint(0, 16, (1, MN), generator=g)
+        W.append((q * 0.002 * (0.5 + torch.rand(MKK // 128, 1, MN, generator=g)).repeat_interleave(128, 0).view(MKK, MN)).to(dt))
+    xr = torch.randn(MT, MK, MKK, generator=g)
+    xr[..., torch.randperm(MKK, generator=g)[:MKK // 100]] *= 20.0
+    ids = torch.stack([torch.randperm(ME, generator=g)[:MK] for _ in range(MT)]) if ids is None else ids
+    w = torch.softmax(torch.randn(MT, MK, generator=g), -1) if w is None else w
+    return {"dt": dt, "W": W, "xr": xr.to(dt), "ids": ids, "w": w}
+
+
+def _moe_exact(c):
+    rows = [(c["xr"][t, s].double(), c["W"][int(c["ids"][t, s])].double()) for t in range(MT) for s in range(MK)]
+    return torch.stack([x @ Wd for x, Wd in rows]), torch.stack([x.abs() @ Wd.abs() for x, Wd in rows])   # [T * k, N]
+
+
+def _moe_slots(c, chunk=128, skip_group=None):
+    """v [T, k, N]: every slot's fp32 sum in chunks of `chunk` channels, rounded to T.  skip_group = (t, s, g, block): channels
+    g * 128 .. + 127 left out of slot (t, s)'s sum in the 128 columns of `block`."""
+    v = torch.zeros(MT, MK, MN)
+    for t in range(MT):
+        for s in range(MK):
+            x, Wf = c["xr"][t, s].float(), c["W"][int(c["ids"][t, s])].float()
+            for k0 in range(0, MKK, chunk):
+                p = x[k0:k0 + chunk] @ Wf[k0:k0 + chunk]
+                if skip_group is not None and skip_group[:2] == (t, s) and k0 // 128 == skip_group[2]:
+                    p[128 * skip_group[3]:128 * skip_group[3] + 128] = 0.0
+                v[t, s] += p
+    return v.to(c["dt"]).float()
+
+
+def _moe_combine(v, w, order=range(MK), skip=()):
+    """out [T, N] = fp32 sum over slots in `order` of fp32(v * w), from 0 (slots (t, s) in `skip` left out)."""
+    out = torch.zeros(MT, MN)
+    for t in range(MT):
+        acc = torch.zeros(MN)
+        for s in order:
+            if (t, s) not in skip:
+                acc = acc + v[t, s] * w[t, s]
+        out[t] = acc
+    return out
+
+
+def _moe_check(c, y, exact):
+    ys, mag = exact
+    return check_combine(y, torch.arange(MT).repeat_interleave(MK), c["w"].reshape(-1), ys, mag)
+
+
+def _passes_old_bounds(c, bad, exact):
+    """The normwise (2e-3) and per-row (2e-3, and so 1.5e-2) bounds of the MoE block's oracle comparisons, against the oracle's
+    combine: fp64 sum of w * T(y_s), rounded to T."""
+    ref = (c["w"].double()[..., None] * exact[0].view(MT, MK, MN).to(c["dt"]).double()).sum(1).to(c["dt"])
+    return _rel(bad, ref) < 2e-3 and all(_rel(bad[t], ref[t]) < 2e-3 for t in range(MT))
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_accepts_any_fp32_order(dt):
+    c = _moe(dt, seed=0)
+    c["w"][1, 2] = 0.0                                                                        # a zero weight
+    exact = _moe_exact(c)
+    for chunk in (16, 128, MKK):
+        v = _moe_slots(c, chunk)
+        for order in ([0, 1, 2, 3], [3, 2, 1, 0], [2, 0, 3, 1]):
+            assert _moe_check(c, _moe_combine(v, c["w"], order).to(dt), exact) <= 1.0, (chunk, order)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_token_without_slot_must_be_zero(dt):
+    c = _moe(dt, seed=4)
+    ys, mag = _moe_exact(c)
+    keep = torch.arange(MT).repeat_interleave(MK) != 3                                        # token 3: every id dropped
+    y = _moe_combine(_moe_slots(c), c["w"], skip={(3, s) for s in range(MK)}).to(dt)
+    assert check_combine(y, torch.arange(MT).repeat_interleave(MK)[keep], c["w"].reshape(-1)[keep], ys[keep], mag[keep]) <= 1.0
+    y[3, 700] = 2.0 ** -20
+    with pytest.raises(AssertionError, match=r"1 of 4096 elements.*\n.*token 3, col 700, block 5\).*no valid slot"):
+        check_combine(y, torch.arange(MT).repeat_interleave(MK)[keep], c["w"].reshape(-1)[keep], ys[keep], mag[keep])
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_flags_one_group_missing_from_one_slot(dt):
+    # token 2's slot 3 (weight 0.01) loses channels 640..767 in column block 3: a dropped K slice of one expert
+    c = _moe(dt, seed=1)
+    c["w"][2] = torch.tensor([0.55, 0.43, 0.01, 0.01])
+    exact = _moe_exact(c)
+    bad = _moe_combine(_moe_slots(c, skip_group=(2, 3, 5, 3)), c["w"]).to(dt)
+    assert _passes_old_bounds(c, bad, exact)
+    with pytest.raises(AssertionError, match=r"elements outside the element-wise bound\n.*token 2, col \d+, block 3\)"):
+        _moe_check(c, bad, exact)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_flags_duplicate_slot_counted_once(dt):
+    # token 1 routes slots 1 and 2 to expert 2; the block adds only the first of them
+    ids = torch.tensor([[0, 1, 2, 3], [0, 2, 2, 3], [3, 2, 1, 0], [1, 0, 3, 2]])
+    c = _moe(dt, seed=2, ids=ids)
+    c["w"][1] = torch.tensor([0.55, 0.00005, 0.0006, 0.44935])
+    c["xr"][1, 2] = c["xr"][1, 1]                                                           # one h row feeds both duplicates
+    exact = _moe_exact(c)
+    bad = _moe_combine(_moe_slots(c), c["w"], skip={(1, 2)}).to(dt)
+    assert _passes_old_bounds(c, bad, exact)
+    with pytest.raises(AssertionError, match=r"elements outside the element-wise bound\n.*token 1, col"):
+        _moe_check(c, bad, exact)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_flags_slot_0_weight_on_slot_1(dt):
+    c = _moe(dt, seed=3)
+    c["w"][0] = torch.tensor([0.0204, 0.02, 0.5, 0.4596])
+    exact = _moe_exact(c)
+    wrong = c["w"].clone()
+    wrong[0, 1] = wrong[0, 0]                                                               # token 0: slot 1 added with slot 0's weight
+    bad = _moe_combine(_moe_slots(c), wrong).to(dt)
+    assert _passes_old_bounds(c, bad, exact)
+    with pytest.raises(AssertionError, match=r"elements outside the element-wise bound\n.*token 0, col"):
+        _moe_check(c, bad, exact)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_moe_bound_flags_three_ulps_on_one_element(dt):
+    c = _moe(dt, seed=5)
+    exact = _moe_exact(c)
+    y = _moe_combine(_moe_slots(c), c["w"]).to(dt)
+    t, n = divmod(int(y.float().abs().argmax()), MN)
+    bad = y.clone()
+    bad[t, n] = (y[t, n].double() + 3 * ulp(y[t, n].double(), dt)).to(dt)
+    assert _passes_old_bounds(c, bad, exact)
+    assert _moe_check(c, y, exact) <= 1.0
+    with pytest.raises(AssertionError, match=f"1 of 4096 elements.*\n.*token {t}, col {n}, block {n // 128}\\)"):
+        _moe_check(c, bad, exact)
