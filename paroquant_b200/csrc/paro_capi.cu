@@ -1,6 +1,7 @@
 // extern "C" surface of libparo_b200.so (declared in include/paro_b200.h): argument checks with
 // the reference's error behaviour (TORCH_CHECK -> message, here: code + paro_last_error()),
 // dispatch to the sm_90a kernels.  No allocation, no host synchronisation.
+#include <atomic>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -57,14 +58,42 @@ int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const
 int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, int32_t *out);
 int moe_debug_silu_mul(int dtype, const void *gate_up, void *act, int64_t M, int I, cudaStream_t stream);
 
-// rows up to which the persistent small-M kernel serves a linear; above, the rotation pre-pass + GEMM path (knob for A/B runs)
-static int small_m_max() {
-  static const int v = [] {
-    const char *e = getenv("PARO_SMALL_M_MAX");
-    const int n = e && *e ? atoi(e) : 16;
-    return n < 0 ? 0 : n > 16 ? 16 : n;
+const Knobs &knobs() {
+  static const Knobs k = [] {
+    auto env = [](const char *name, int dflt) {
+      const char *v = getenv(name);
+      return v && *v ? atoi(v) : dflt;
+    };
+    Knobs x;
+    const int m = env("PARO_SMALL_M_MAX", 16);
+    x.small_m_max = m < 0 ? 0 : m > 16 ? 16 : m;
+    x.decode_stream = env("PARO_DECODE_STREAM", 0) != 0;
+    x.prerot_m = env("PARO_DECODE_PREROT_M", 0);
+    x.no_cluster = env("PARO_NO_CLUSTER", 0);
+    x.force_c = env("PARO_DECODE_C", 0);
+    x.stages = env("PARO_DECODE_STAGES", 0);
+    x.inflight = env("PARO_DECODE_INFLIGHT", 6);
+    x.b8 = env("PARO_DECODE_B8", 1);
+    x.no_pdl = env("PARO_NO_PDL", 0);
+    x.trace = env("PARO_DECODE_TRACE", 0);
+    x.verbose = env("PARO_DECODE_VERBOSE", 0);
+    return x;
   }();
-  return v;
+  return k;
+}
+
+int device_sms() {
+  static std::atomic<int> sms_of[64];   // per device; threads that race on a first query store the same value
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (dev < 64) {
+    const int n = sms_of[dev].load(std::memory_order_relaxed);
+    if (n) return n;
+  }
+  int n = 0;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
+  if (dev < 64) sms_of[dev].store(n, std::memory_order_relaxed);
+  return n;
 }
 
 static bool valid_dtype(int d) { return d == PARO_F32 || d == PARO_F16 || d == PARO_BF16; }
@@ -150,7 +179,7 @@ size_t paro_workspace_bytes(const paro_linear_shape *shape, int64_t max_m) {
     const size_t d = stream_sync_bytes(L) + decode_scratch_bytes(L, max_m);
     if (d > b) b = d;
   }
-  if (max_m > small_m_max()) {
+  if (max_m > knobs().small_m_max) {
     const size_t g = stream_sync_bytes(L) + gemm_workspace_bytes(L, max_m);
     if (g > b) b = g;
   }
@@ -171,13 +200,12 @@ int paro_linear_forward(const paro_linear_shape *shape, const void *packed, cons
     return PARO_EINVAL;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (M <= small_m_max()) {
+  if (M <= knobs().small_m_max) {
     // A single linear: the cluster kernel (paro_decode.cu: K slices reduced through distributed shared memory) has the shorter
     // tail -- measured 7.4 / 9.9 / 22.0 / 15.6 us on the Llama-3-8B shapes at M = 1 against 11.1 / 12.3 / 24.3 / 16.2 us for
     // the chain kernel run as a one-step chain, whose cross-CTA sums travel through L2.  The chain kernel takes over where the
     // cluster kernel has no launch plan (very long K) and for chains / tensor-parallel steps (paro_chain_forward).
-    static const bool stream_only = [] { const char *v = getenv("PARO_DECODE_STREAM"); return v && *v && atoi(v) != 0; }();
-    if (!stream_only) {
+    if (!knobs().decode_stream) {
       const size_t head = stream_sync_bytes(L);   // the pre-rotated rows of the M >= 4 pre-pass live behind the epoch word
       const int rc = decode_forward(*shape, L, packed, x, M, bias, y, static_cast<uint8_t *>(workspace) + head,
                                     workspace_bytes > head ? workspace_bytes - head : 0, st);

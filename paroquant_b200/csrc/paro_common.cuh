@@ -24,6 +24,50 @@ void note_launches(int n);
     }                                                                                        \
   } while (0)
 
+// Every PARO_* environment knob the library reads, read once per process (paro_capi.cu)
+struct Knobs {
+  int small_m_max;     // PARO_SMALL_M_MAX (0..16, default 16): rows up to which the small-M kernels serve a linear
+  int decode_stream;   // PARO_DECODE_STREAM: a single linear takes the chain kernel, not the cluster kernel
+  int prerot_m;        // PARO_DECODE_PREROT_M: 0 the built-in rule, n >= 2 pre-rotate from n rows on, 1 never
+  int no_cluster;      // PARO_NO_CLUSTER: the cluster kernel runs without clusters
+  int force_c;         // PARO_DECODE_C: K slices per linear (0: planned)
+  int stages;          // PARO_DECODE_STAGES: ring depth cap (0: as deep as shared memory allows)
+  int inflight;        // PARO_DECODE_INFLIGHT (default 6): the chain kernel's bulk copies outstanding per SM
+  int b8;              // PARO_DECODE_B8 (default 1): the chain kernel stores 8 B-operand rows for M <= 8
+  int no_pdl;          // PARO_NO_PDL: the small-M kernels launch without programmatic dependent launch
+  int trace;           // PARO_DECODE_TRACE: the small-M kernels write their phase timestamps
+  int verbose;         // PARO_DECODE_VERBOSE: the small-M kernels print their launch plans
+};
+const Knobs &knobs();
+
+// SM count of the current device, asked once per device; 0 without a device
+int device_sms();
+
+// cfg for `grid` CTAs of `threads` threads with `smem` bytes of dynamic shared memory; attr (cfg points at it) gets a cluster
+// dimension of `cluster` CTAs when cluster > 0 and programmatic stream serialization when pdl
+inline void launch_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute (&attr)[2], int grid, int threads, size_t smem, cudaStream_t stream,
+                          int cluster, bool pdl) {
+  cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 0;
+  if (cluster > 0) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+    attr[cfg.numAttrs].val.clusterDim.x = cluster;
+    attr[cfg.numAttrs].val.clusterDim.y = 1;
+    attr[cfg.numAttrs].val.clusterDim.z = 1;
+    ++cfg.numAttrs;
+  }
+  if (pdl) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    ++cfg.numAttrs;
+  }
+}
+
 // ------------------------------------------------------------------ dtype traits
 // Every conversion below is one round-to-nearest-even, matching rotation.cuh's Traits
 // (/root/reference/paroquant/kernels/cuda/rotation.cuh:177-205).

@@ -72,93 +72,6 @@ struct DecParams {
   long long meta_off, rec_off;
 };
 
-// ---- prologue.  A rotation TASK = (group gi of the CTA's slice, block of up to ROWS <= 4 token rows); worker warp w takes
-// tasks w, w + W, ...  (M = 16: four tasks per group, so all warps share the rotation instead of 16-row tiles on a few).
-// B[gi][k16 step s][k half h][row m][8 k]: 16 rows x 16 bytes per core-matrix pair, 512 bytes per step.
-template <typename T, int ROWS>
-__device__ __forceinline__ void dec_write_b_rows(uint32_t xb_group, uint32_t rot, int m0, int nrows, int lane) {
-  for (int idx = lane; idx < 16 * nrows; idx += 32) {
-    const int ml = idx >> 4, s = (idx >> 1) & 7, h = idx & 1;
-    const int c0 = 16 * s + 8 * h, m = m0 + ml;
-    uint4 v;
-    if constexpr (ROWS == 1) {
-      v = lds128(rot + c0 * 2);
-    } else {
-      uint32_t e[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) e[k] = lds16(rot + (c0 + k) * (ROWS * 2) + 2 * ml);
-      v = make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
-    }
-    sts128u(xb_group + s * (kDecN * 32) + h * (kDecN * 16) + (m >> 3) * 128 + (m & 7) * 16, v);
-  }
-}
-struct DecRotMeta {
-  uint32_t idxw[8], tw[8];
-  uint2 csw;
-  const uint8_t *meta;
-};
-
-__device__ __forceinline__ void dec_fetch_meta(const DecParams &p, int part, int gk, int lane, DecRotMeta &rm) {
-  rm.meta = p.packed + p.meta_off + (static_cast<size_t>(part) * p.groups + gk) * p.meta_group_bytes;
-  if (p.pre_rotated) return;   // no rotation tasks at all
-  rm.csw = *reinterpret_cast<const uint2 *>(rm.meta + p.krot * 256 + 8 * lane);
-  if (p.krot == 8) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      rm.idxw[r] = *reinterpret_cast<const uint32_t *>(rm.meta + r * 128 + 4 * lane);
-      rm.tw[r] = *reinterpret_cast<const uint32_t *>(rm.meta + 8 * 128 + r * 128 + 4 * lane);
-    }
-  }
-}
-
-template <typename T, int ROWS>
-__device__ __forceinline__ void dec_rotate_task(const DecParams &p, const DecRotMeta &rm, const void *xpart, int gk, int m0, int lane, uint32_t rot,
-                                                uint32_t xb_group, long long t_entry) {
-  uint2 raw[ROWS];
-  struct { const void *x; int M, K; } px = {xpart, p.M, p.K};   // my partition's rows (a pre-rotated x has one copy per partition)
-  load_x<T, ROWS>(px, gk, lane, raw, m0);
-  scale_and_stage<T, ROWS>(rot, lane, raw, rm.csw);
-  __syncwarp();
-  if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 0] = clock64() - t_entry;
-  if (p.krot == 8) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      // (keeping all 32 coefficients live across griddepcontrol.wait was tried: it spills at 80 registers and the
-      // stages get slower than with the MUFU work inline)
-      float c0, s0, c1, s1;
-      sincos2<T>(rm.tw[r], c0, s0, c1, s1);
-      rotate_stage<T, ROWS>(rot, rm.idxw[r], c0, s0, c1, s1);
-      __syncwarp();
-    }
-  } else {
-    const int krot = p.krot;
-    for (int r = 0; r < krot; ++r) {
-      const uint32_t iw = *reinterpret_cast<const uint32_t *>(rm.meta + r * 128 + 4 * lane);
-      const uint32_t tw = *reinterpret_cast<const uint32_t *>(rm.meta + krot * 128 + r * 128 + 4 * lane);
-      float c0, s0, c1, s1;
-      sincos2<T>(tw, c0, s0, c1, s1);
-      rotate_stage<T, ROWS>(rot, iw, c0, s0, c1, s1);
-      __syncwarp();
-    }
-  }
-  if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 9] = clock64() - t_entry;
-  const int left = p.M - m0;
-  dec_write_b_rows<T, ROWS>(xb_group, rot, m0, left < ROWS ? left : ROWS, lane);
-  __syncwarp();
-}
-
-// tasks t = wi, wi + nwarps, ... of ng * nq (nq row blocks per group); the first task's metadata was fetched before the wait
-template <typename T, int ROWS>
-__device__ __forceinline__ void dec_prologue(const DecParams &p, DecRotMeta &rm, int part, int g_begin, int ntasks, int nq, int wi, int nwarps,
-                                             int lane, uint32_t rot, uint32_t xb, long long t_entry) {
-  const void *xpart = static_cast<const T *>(p.x) + static_cast<long long>(part) * p.x_part_stride;
-  for (int t = wi; t < ntasks; t += nwarps) {
-    const int gi = t / nq, rq = t - gi * nq;
-    if (t != wi) dec_fetch_meta(p, part, g_begin + gi, lane, rm);
-    dec_rotate_task<T, ROWS>(p, rm, xpart, g_begin + gi, rq * ROWS, lane, rot, xb + gi * (kDecN * 256), t_entry);
-  }
-}
-
 template <typename T>
 __device__ __forceinline__ void dec_store(const DecParams &p, float v, int m, int n) {
   T t = Traits<T>::from_float(v);
@@ -202,10 +115,13 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
   const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
   const uint8_t *rec0 = p.packed + p.rec_off + (static_cast<size_t>(p.part_block_begin[part] + cb_begin) * p.groups + g_begin) * rec_bytes;
 
-  DecRotMeta rm;
-  const int nq = p.M > 4 ? (p.M + 3) >> 2 : 1, ntasks = ng * nq;   // rotation tasks: row blocks of 4 for M > 4
-  if (warp < kWorkers && warp < ntasks && warp < p.rot_warps)
-    dec_fetch_meta(p, part, g_begin + warp / nq, lane, rm);   // flies during the barrier initialisation
+  // A rotation task = (group of the slice, block of up to 4 token rows); worker warp w takes tasks w, w + rot_warps, ...  (M = 16:
+  // four tasks per group, so all warps share the rotation instead of 16-row tiles on a few)
+  RotMeta rm;
+  const int nq = p.M > 4 ? (p.M + 3) >> 2 : 1, ntasks = ng * nq;
+  const int mi0 = part * p.groups + g_begin;   // metadata block of the slice's first group
+  if (!p.pre_rotated && warp < kWorkers && warp < ntasks && warp < p.rot_warps)
+    fetch_meta(p.packed + p.meta_off + static_cast<size_t>(mi0 + warp / nq) * p.meta_group_bytes, p.krot, lane, rm);   // flies during the barrier initialisation
 
   if (warp == kWorkers) {
     // one barrier per lane; every worker warp consumes every ring stage
@@ -269,9 +185,23 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
       if (wi < ntasks && wi < p.rot_warps) {
         const uint32_t rot = smem0 + p.rot_off + wi * p.rot_bytes;
         const int M = p.M, rw = p.rot_warps;
-        if (M == 1) dec_prologue<T, 1>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
-        else if (M == 2) dec_prologue<T, 2>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
-        else dec_prologue<T, 4>(p, rm, part, g_begin, ntasks, nq, wi, rw, lane, rot, xb, t_entry);
+        const uint8_t *meta = p.packed + p.meta_off;
+        auto stage_x = [&](auto rows, int gi, int m0, uint2 csw) {
+          constexpr int ROWS = decltype(rows)::value;
+          const T *xg = static_cast<const T *>(p.x) + (g_begin + gi) * kGroup + 4 * lane;
+          uint2 raw[ROWS];
+#pragma unroll
+          for (int m = 0; m < ROWS; ++m) {
+            raw[m] = make_uint2(0u, 0u);
+            if (m0 + m < M) raw[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * p.K));
+          }
+          scale_and_stage<T, ROWS>(rot, lane, raw, csw);
+          if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 0] = clock64() - t_entry;
+        };
+        if (M == 1) rotation_tasks<T, 1, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        else if (M == 2) rotation_tasks<T, 2, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        else rotation_tasks<T, 4, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 9] = clock64() - t_entry;
       }
       named_bar_sync(2, 32 * kWorkers);   // B operand complete
     }
@@ -406,68 +336,23 @@ int decode_trace_read(unsigned long long *host, int max_ctas) {
 }
 
 // ------------------------------------------------------------------ host side
-static int dec_env_int(const char *name, int dflt) {
-  const char *v = getenv(name);
-  return v && *v ? atoi(v) : dflt;
-}
-// environment knobs are read ONCE per process (every launch used to pay half a dozen getenv calls)
-struct DecKnobs { int stages, no_cluster, force_c, verbose, no_pdl, trace; };
-static const DecKnobs &dec_knobs() {
-  static const DecKnobs k = {dec_env_int("PARO_DECODE_STAGES", 0), dec_env_int("PARO_NO_CLUSTER", 0), dec_env_int("PARO_DECODE_C", 0),
-                             dec_env_int("PARO_DECODE_VERBOSE", 0), dec_env_int("PARO_NO_PDL", 0), dec_env_int("PARO_DECODE_TRACE", 0)};
-  return k;
-}
-
 struct DecPlan {
   int c, c_shift, ranges, grid;
   int part_range_begin[PARO_MAX_PARTS + 1];
   int nj_max, ng_max;
 };
 
-// `ranges` block ranges over the partitions, proportional to their 128-column block counts (largest remainder)
+// `ranges` block ranges over the partitions, proportional to their 128-column blocks, at most one per block
 static bool dec_split_ranges(const Layout &L, int ranges, DecPlan &plan) {
-  int cb[PARO_MAX_PARTS], alloc[PARO_MAX_PARTS], total = 0;
-  double frac[PARO_MAX_PARTS];
-  for (int p = 0; p < L.n_parts; ++p) {
-    cb[p] = L.part_block_begin[p + 1] - L.part_block_begin[p];
-    total += cb[p];
-  }
-  if (ranges > total) ranges = total;
-  if (ranges < L.n_parts) return false;
-  int used = 0;
-  for (int p = 0; p < L.n_parts; ++p) {
-    const double exact = static_cast<double>(ranges) * cb[p] / total;
-    alloc[p] = static_cast<int>(exact);
-    if (alloc[p] < 1) alloc[p] = 1;
-    if (alloc[p] > cb[p]) alloc[p] = cb[p];
-    frac[p] = exact - alloc[p];
-    used += alloc[p];
-  }
-  while (used < ranges) {
-    int best = -1;
-    for (int p = 0; p < L.n_parts; ++p)
-      if (alloc[p] < cb[p] && (best < 0 || frac[p] > frac[best])) best = p;
-    if (best < 0) break;
-    alloc[best]++; frac[best] -= 1.0; used++;
-  }
-  while (used > ranges) {
-    int best = -1;
-    for (int p = 0; p < L.n_parts; ++p)
-      if (alloc[p] > 1 && (best < 0 || frac[p] < frac[best])) best = p;
-    if (best < 0) return false;
-    alloc[best]--; frac[best] += 1.0; used--;
-  }
-  plan.part_range_begin[0] = 0;
+  if (!apportion(L, ranges < L.blocks_total ? ranges : L.blocks_total, plan.part_range_begin)) return false;
   plan.nj_max = 0;
-  for (int p = 0; p < PARO_MAX_PARTS; ++p) {
-    plan.part_range_begin[p + 1] = plan.part_range_begin[p] + (p < L.n_parts ? alloc[p] : 0);
-    if (p < L.n_parts) {
-      const int mx = (cb[p] + alloc[p] - 1) / alloc[p];
-      if (mx > plan.nj_max) plan.nj_max = mx;
-    }
+  for (int p = 0; p < L.n_parts; ++p) {
+    const int cb = L.part_block_begin[p + 1] - L.part_block_begin[p], n = plan.part_range_begin[p + 1] - plan.part_range_begin[p];
+    const int mx = (cb + n - 1) / n;
+    if (mx > plan.nj_max) plan.nj_max = mx;
   }
   plan.ranges = plan.part_range_begin[L.n_parts];
-  return plan.ranges > 0;
+  return true;
 }
 
 struct DecSmem { int xb_off, rot_off, recv_off, bar_off, nstages, rot_warps, total; };
@@ -480,7 +365,7 @@ static bool dec_carve_with(const DecPlan &plan, int M, int rot_bytes, int sets, 
   const int fixed = xb_bytes + rot_total + recv + bar_bytes + 128;
   int nst = (kDecSmemLimit - fixed) / stage_bytes;
   if (nst > kDecMaxStages) nst = kDecMaxStages;
-  const int want = dec_knobs().stages;
+  const int want = knobs().stages;
   if (want >= sets && want < nst) nst = want;
   nst = nst / sets * sets;   // a stage is always consumed by the same set
   if (nst < sets) return false;
@@ -513,17 +398,9 @@ static int max_resident_clusters(int c, int smem_bytes, int sms) {
   while ((1 << slot) < c) ++slot;
   auto kern = decode_kernel<T>;
   if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) { (void)cudaGetLastError(); return 0; }   // never lowered: cached plans keep launching
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((sms / c) * c);
-  cfg.blockDim = dim3(32 * (kDecWorkers + 1));
-  cfg.dynamicSmemBytes = smem_bytes;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = c;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[2];
+  launch_config(cfg, attr, (sms / c) * c, 32 * (kDecWorkers + 1), smem_bytes, 0, c, false);
   int n = 0;
   if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
   return n;   // (the caller caches the whole plan per shape, M and device)
@@ -588,7 +465,7 @@ struct DecCached { bool found; DecPlan plan; DecSmem smem; };
 template <typename T>
 static DecCached dec_cached_plan(const Layout &L, int M, int sms) {
   auto kern = decode_kernel<T>;
-  const DecKnobs &kn = dec_knobs();
+  const Knobs &kn = knobs();
   struct Key {
     int K, N, krot, n_parts, M, dev, qhalves, parts[PARO_MAX_PARTS];
     bool operator<(const Key &o) const { return memcmp(this, &o, sizeof(Key)) < 0; }
@@ -622,34 +499,16 @@ static DecCached dec_cached_plan(const Layout &L, int M, int sms) {
 template <typename T>
 static int launch_decode(DecParams &p, const Layout &L, const DecCached &c, cudaStream_t stream) {
   auto kern = decode_kernel<T>;
-  const DecKnobs &kn = dec_knobs();
+  const Knobs &kn = knobs();
   const DecPlan &best = c.plan;
   const DecSmem &best_s = c.smem;
   if (kn.verbose)
     fprintf(stderr, "[paro decode] K=%d N=%d M=%d: cluster %d x %d ranges (grid %d), blocks/CTA <= %d, groups/CTA <= %d, %d stages, smem %d\n",
             L.K, L.N, p.M, best.c, best.ranges, best.grid, best.nj_max, best.ng_max, best_s.nstages, best_s.total);
 
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(best.grid);
-  cfg.blockDim = dim3(32 * (kDecWorkers + 1));
-  cfg.dynamicSmemBytes = best_s.total;
-  cfg.stream = stream;
+  cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (best.c > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = best.c;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (!kn.no_pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
+  launch_config(cfg, attr, best.grid, 32 * (kDecWorkers + 1), best_s.total, stream, best.c > 1 ? best.c : 0, !kn.no_pdl);
   p.c = best.c; p.c_shift = best.c_shift;
   p.nstages = best_s.nstages;
   p.rot_warps = best_s.rot_warps;
@@ -668,12 +527,8 @@ bool decode_supported(const Layout &L, int64_t M) { return M >= 1 && M <= 16 && 
 // at M = 16 a CTA has 32-56 of them: 28 k of o_proj's 40 k cycles, 48 k of down_proj's 80 k (tools/trace_decode.py).  Measured
 // (us, in-kernel -> pre-pass): M = 16: o 21.7 -> 13.4, qkv 18.2 -> 16.4, gate_up 38.1 -> 29.1, down 42.3 -> 23.8; M = 8: 14.0 ->
 // 11.8, 16.7 -> 15.0, 29.7 -> 27.5, 38.2 -> 20.3; M = 4: o 10.0 -> 11.4 (stays in-kernel), down 25.1 -> 18.7.
-static int dec_prerot_knob() {
-  static const int v = dec_env_int("PARO_DECODE_PREROT_M", 0);   // 0: the rule below; n >= 2: from n rows on; 1: never
-  return v;
-}
 static bool decode_wants_prerot(const Layout &L, int64_t M) {
-  const int k = dec_prerot_knob();
+  const int k = knobs().prerot_m;   // 0: the rule below; n >= 2: from n rows on; 1: never
   if (k == 1) return false;
   if (k >= 2) return M >= k;
   return M >= 5 || (M >= 3 && L.groups >= 64);
@@ -689,11 +544,8 @@ int rotate_small_launch(const void *x, void *out, const void *raw_base, long lon
 
 int decode_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
                    const void *bias, void *y, void *scratch, size_t scratch_bytes, cudaStream_t stream) {
-  int dev = 0;
-  PARO_CUDA_OK(cudaGetDevice(&dev));
-  static thread_local int sms_of[64] = {};   // SM count per device, asked once
-  if (!sms_of[dev & 63]) PARO_CUDA_OK(cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  const int sms = sms_of[dev & 63];
+  const int sms = device_sms();
+  if (sms <= 0) { set_error("decode: no CUDA device"); return PARO_ECUDA; }
   // no plan (e.g. K too long for one CTA without clusters): the caller falls back to the stream kernel, before any launch
   const DecCached plan = s.dtype == PARO_BF16 ? dec_cached_plan<__nv_bfloat16>(L, static_cast<int>(M), sms)
                                               : dec_cached_plan<__half>(L, static_cast<int>(M), sms);
@@ -714,7 +566,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   p.n_parts = L.n_parts; p.groups = L.groups; p.krot = L.krot;
   p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2;
   p.rot_bytes = dec_rot_bytes(M);
-  p.trace = dec_knobs().trace;
+  p.trace = knobs().trace;
   for (int i = 0; i <= PARO_MAX_PARTS; ++i) {
     p.part_col_begin[i] = L.part_col_begin[i];
     p.part_block_begin[i] = L.part_block_begin[i];

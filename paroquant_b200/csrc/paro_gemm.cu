@@ -215,15 +215,6 @@ static int pick_nt(int64_t M, const Layout &L, int sms) {
   return best;
 }
 
-static int gemm_device_sms() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
-  }
-  return sms;
-}
-
 // test hook: out[0] = tokens per tile (NT), out[1] = token blocks
 int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out) {
   if (M < 1 || sms < 1) { set_error("debug_gemm_plan: bad M / sms"); return PARO_EINVAL; }
@@ -243,16 +234,9 @@ static int launch_gemm(const GemmParams &p, cudaStream_t stream) {
   auto kern = wg_gemm_kernel<T, NT>;
   const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256;
   PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(p.n_blocks * p.tok_blocks);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;  // prologue + first weight stages overlap the pre-pass
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[2];
+  launch_config(cfg, attr, p.n_blocks * p.tok_blocks, kGemmThreads, smem, stream, 0, true);   // PDL: prologue + first weight stages overlap the pre-pass
   PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
   note_launches(1);
   return PARO_OK;
@@ -271,7 +255,8 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
     set_error("workspace too small: have %zu, need %zu", workspace_bytes, gemm_workspace_bytes(L, M));
     return PARO_EWORKSPACE;
   }
-  const int NT = pick_nt(M, L, gemm_device_sms());
+  const int sms = device_sms();
+  const int NT = pick_nt(M, L, sms > 0 ? sms : 132);
   const int64_t m_pad = (M + NT - 1) / NT * NT;
   const uint8_t *pk = static_cast<const uint8_t *>(packed);
   uint8_t *xr_base = static_cast<uint8_t *>(workspace);

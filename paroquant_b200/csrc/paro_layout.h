@@ -124,4 +124,36 @@ inline bool make_layout(const paro_linear_shape &s, Layout &L, const char **why)
   return true;
 }
 
+// `count` units (CTAs, block ranges) dealt to the partitions in proportion to their 128-column blocks, at least one each
+// (largest remainder): partition p gets begin[p] .. begin[p + 1] - 1.  False if count < n_parts.
+inline bool apportion(const Layout &L, int count, int *begin) {
+  int alloc[PARO_MAX_PARTS];
+  double frac[PARO_MAX_PARTS];
+  if (count < L.n_parts) return false;
+  int used = 0;
+  for (int p = 0; p < L.n_parts; ++p) {
+    const double exact = static_cast<double>(count) * (L.part_block_begin[p + 1] - L.part_block_begin[p]) / L.blocks_total;
+    alloc[p] = static_cast<int>(exact);
+    if (alloc[p] < 1) alloc[p] = 1;
+    frac[p] = exact - alloc[p];
+    used += alloc[p];
+  }
+  while (used < count) {
+    int best = 0;
+    for (int p = 1; p < L.n_parts; ++p)
+      if (frac[p] > frac[best]) best = p;
+    alloc[best]++; frac[best] -= 1.0; used++;
+  }
+  while (used > count) {
+    int best = -1;
+    for (int p = 0; p < L.n_parts; ++p)
+      if (alloc[p] > 1 && (best < 0 || frac[p] < frac[best])) best = p;
+    if (best < 0) return false;
+    alloc[best]--; frac[best] += 1.0; used--;
+  }
+  begin[0] = 0;
+  for (int p = 0; p < PARO_MAX_PARTS; ++p) begin[p + 1] = begin[p] + (p < L.n_parts ? alloc[p] : 0);
+  return true;
+}
+
 }  // namespace paro

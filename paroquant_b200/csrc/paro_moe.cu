@@ -6,9 +6,9 @@
 //   launch 2 (down):     y_s      = T(rotate_d(T(T(silu(gate)) * up)) . W_d[e_s])
 //                        out[t]   = T(sum over (expert id, slot) ascending of fp32(y_s) * w_s, from 0, product rounded first)
 //
-// Both launches are one kernel template built from decode_kernel's pieces (paro_decode.cu): 16 worker warps (8 row tiles x 2
-// k halves, mma.sync with dequantised A fragments in registers, B = rotated token rows in shared memory) and a TMA producer
-// warp streaming ONE record per ring stage.
+// Both launches are one kernel template built from decode_kernel's pieces (paro_tc_common.cuh): 16 worker warps (8 row tiles x 2
+// k halves, mma.sync with dequantised A fragments in registers, B = token rows rotated by rotation_tasks in shared memory) and
+// a TMA producer warp streaming ONE record per ring stage.
 //
 // Routing.  After griddepcontrol.wait every CTA ranks the T * k <= 128 ids in shared memory: the ascending list of distinct
 // valid experts u = 0..U-1 (ids outside [0, E) are dropped) and, per (u, token), the mask of slots that chose it.  The launch
@@ -71,64 +71,6 @@ PARO_HD inline int moe_waves(int U, int S, int c) { return (U * S + c - 1) / c; 
 __device__ __forceinline__ int nth_bit(uint32_t mask, int m) {
   for (int j = 0; j < m; ++j) mask &= mask - 1;
   return __ffs(mask) - 1;
-}
-
-// B[gi][k16 step s][k half h][row m][8 k] of rows m0 .. m0 + nrows - 1 from a rotation tile (as dec_write_b_rows)
-template <typename T, int ROWS>
-__device__ __forceinline__ void moe_write_b_rows(uint32_t xb_group, uint32_t rot, int m0, int nrows, int lane) {
-  for (int idx = lane; idx < 16 * nrows; idx += 32) {
-    const int ml = idx >> 4, s = (idx >> 1) & 7, h = idx & 1;
-    const int c0 = 16 * s + 8 * h, m = m0 + ml;
-    uint4 v;
-    if constexpr (ROWS == 1) {
-      v = lds128(rot + c0 * 2);
-    } else {
-      uint32_t e[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) e[k] = lds16(rot + (c0 + k) * (ROWS * 2) + 2 * ml);
-      v = make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
-    }
-    sts128u(xb_group + s * (kMoeN * 32) + h * (kMoeN * 16) + (m >> 3) * 128 + (m & 7) * 16, v);
-  }
-}
-
-// One rotation task: rows m0 .. m0 + ROWS - 1 of the expert's row list (tokens of `tokmask`, ascending) for group gk.
-// Launch 1 reads x[t]; launch 2 reads h[t, first slot of t] and applies SiLU * up first.
-template <typename T, int ROWS, bool DOWN>
-__device__ __forceinline__ void moe_rotate_task(const MoeParams &p, const uint8_t *meta, uint32_t tokmask, const uint32_t *umask, int R, int gk,
-                                                int m0, int lane, uint32_t rot, uint32_t xb_group) {
-  uint2 raw[ROWS];
-#pragma unroll
-  for (int j = 0; j < ROWS; ++j) {
-    raw[j] = make_uint2(0u, 0u);
-    if (m0 + j < R) {
-      const int t = nth_bit(tokmask, m0 + j);
-      if constexpr (DOWN) {
-        const int slot = __ffs(umask[t]) - 1;   // duplicate slots of one token carry the same h row
-        const T *row = static_cast<const T *>(p.x) + (static_cast<int64_t>(t) * p.k + slot) * (2 * p.K) + gk * kGroup + 4 * lane;
-        const uint2 g = __ldcg(reinterpret_cast<const uint2 *>(row)), u = __ldcg(reinterpret_cast<const uint2 *>(row + p.K));
-        raw[j].x = silu_mul2<T>(g.x, u.x);
-        raw[j].y = silu_mul2<T>(g.y, u.y);
-      } else {
-        raw[j] = __ldcg(reinterpret_cast<const uint2 *>(static_cast<const T *>(p.x) + static_cast<int64_t>(t) * p.K + gk * kGroup + 4 * lane));
-      }
-    }
-  }
-  const uint2 csw = *reinterpret_cast<const uint2 *>(meta + p.krot * 256 + 8 * lane);
-  scale_and_stage<T, ROWS>(rot, lane, raw, csw);
-  __syncwarp();
-  const int krot = p.krot;
-  for (int r = 0; r < krot; ++r) {
-    const uint32_t iw = *reinterpret_cast<const uint32_t *>(meta + r * 128 + 4 * lane);
-    const uint32_t tw = *reinterpret_cast<const uint32_t *>(meta + krot * 128 + r * 128 + 4 * lane);
-    float c0, s0, c1, s1;
-    sincos2<T>(tw, c0, s0, c1, s1);
-    rotate_stage<T, ROWS>(rot, iw, c0, s0, c1, s1);
-    __syncwarp();
-  }
-  const int left = R - m0;
-  moe_write_b_rows<T, ROWS>(xb_group, rot, m0, left < ROWS ? left : ROWS, lane);
-  __syncwarp();
 }
 
 template <typename T, bool DOWN>
@@ -241,21 +183,42 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
       const uint32_t *umask = s_mask + u * 16;
       const uint32_t tokmask = __ballot_sync(0xFFFFFFFFu, lane < ntok && umask[lane & 15] != 0u);
       const int R = __popc(tokmask);
-      const uint8_t *pe = p.packed + s_uexp[u] * p.stride;
-      // ---- B operand of the item: zero rows [R, 16), then the rotation tasks (group x block of up to 4 rows)
+      // ---- B operand of the item: zero rows [R, 16), then the rotation tasks (group x block of up to 4 rows) of the expert's
+      // rows: its tokens (`tokmask`) ascending.  Launch 1 reads x[t]; launch 2 reads h[t, first slot of t] and applies SiLU * up.
+      const uint8_t *meta = p.packed + s_uexp[u] * p.stride + p.meta_off;   // partition 0 (gate and up share it)
+      const int nq = R > 4 ? (R + 3) >> 2 : 1, ntasks = ng * nq;
+      RotMeta rm;
+      if (warp < ntasks) fetch_meta<false>(meta + static_cast<size_t>(g0 + warp / nq) * p.meta_group_bytes, p.krot, lane, rm);
       for (int idx = tid; idx < ng * (kMoeN * 16); idx += 32 * kMoeWorkers) sts128u(xb + idx * 16, make_uint4(0u, 0u, 0u, 0u));
       named_bar_sync(1, 32 * kMoeWorkers);
       {
-        const int nq = R > 4 ? (R + 3) >> 2 : 1, ntasks = ng * nq;
         const uint32_t rot = rot0 + warp * 1024;
-        for (int tk = warp; tk < ntasks; tk += kMoeWorkers) {
-          const int gi = tk / nq, rq = tk - gi * nq, gk = g0 + gi;
-          const uint8_t *meta = pe + p.meta_off + static_cast<size_t>(gk) * p.meta_group_bytes;   // partition 0 (gate and up share it)
-          const uint32_t xg = xb + gi * (kMoeN * 256);
-          if (R == 1) moe_rotate_task<T, 1, DOWN>(p, meta, tokmask, umask, R, gk, 0, lane, rot, xg);
-          else if (R == 2) moe_rotate_task<T, 2, DOWN>(p, meta, tokmask, umask, R, gk, 0, lane, rot, xg);
-          else moe_rotate_task<T, 4, DOWN>(p, meta, tokmask, umask, R, gk, rq * 4, lane, rot, xg);
-        }
+        auto stage_x = [&](auto rows, int gi, int m0, uint2 csw) {
+          constexpr int ROWS = decltype(rows)::value;
+          const int gk = g0 + gi;
+          uint2 raw[ROWS];
+#pragma unroll
+          for (int j = 0; j < ROWS; ++j) {
+            raw[j] = make_uint2(0u, 0u);
+            if (m0 + j < R) {
+              const int t = nth_bit(tokmask, m0 + j);
+              if constexpr (DOWN) {
+                const int slot = __ffs(umask[t]) - 1;   // duplicate slots of one token carry the same h row
+                const T *row = static_cast<const T *>(p.x) + (static_cast<int64_t>(t) * p.k + slot) * (2 * p.K) + gk * kGroup + 4 * lane;
+                const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + p.K));
+                raw[j].x = silu_mul2<T>(gate.x, up.x);
+                raw[j].y = silu_mul2<T>(gate.y, up.y);
+              } else {
+                raw[j] = __ldcg(reinterpret_cast<const uint2 *>(static_cast<const T *>(p.x) + static_cast<int64_t>(t) * p.K + gk * kGroup + 4 * lane));
+              }
+            }
+          }
+          scale_and_stage<T, ROWS>(rot, lane, raw, csw);
+        };
+        const int mg = p.meta_group_bytes;
+        if (R == 1) rotation_tasks<T, 1, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
+        else if (R == 2) rotation_tasks<T, 2, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
+        else rotation_tasks<T, 4, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
       }
       named_bar_sync(2, 32 * kMoeWorkers);   // B operand complete
       // ---- rounds: one record per ring stage, accumulated in stream order
@@ -417,14 +380,6 @@ static int moe_check(const paro_moe_desc *d, int64_t T, int32_t k, MoeShapes &ms
   return PARO_OK;
 }
 
-static int moe_sms() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  static thread_local int sms_of[64] = {};
-  if (!sms_of[dev & 63] && cudaDeviceGetAttribute(&sms_of[dev & 63], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
-  return sms_of[dev & 63];
-}
-
 static void moe_fill(MoeParams &p, const Layout &L, const MoePlan &m, const void *packed, size_t stride) {
   p.packed = static_cast<const uint8_t *>(packed);
   p.stride = static_cast<long long>(stride);
@@ -444,20 +399,9 @@ static int moe_launch(const MoeParams &p, const MoePlan &m, cudaStream_t stream)
   auto kern = moe_kernel<T, DOWN>;
   static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMoeSmemLimit);
   PARO_CUDA_OK(attr_rc);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(m.grid);
-  cfg.blockDim = dim3(kMoeThreads);
-  cfg.dynamicSmemBytes = m.smem;
-  cfg.stream = stream;
+  cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = m.c;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
+  launch_config(cfg, attr, m.grid, kMoeThreads, m.smem, stream, m.c, true);   // a cluster launch also at c = 1
   PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
   return PARO_OK;
 }
@@ -475,7 +419,7 @@ int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const
     return PARO_EINVAL;
   }
   if (workspace_bytes < 256) { set_error("moe: workspace too small: have %zu, need 256", workspace_bytes); return PARO_EWORKSPACE; }
-  const int Ti = static_cast<int>(T), umax = ms.E < Ti * k ? ms.E : Ti * k, sms = moe_sms();
+  const int Ti = static_cast<int>(T), umax = ms.E < Ti * k ? ms.E : Ti * k, dev_sms = device_sms(), sms = dev_sms > 0 ? dev_sms : 132;
   MoePlan m1, m2;
   if (!moe_choose_plan(ms.gu, Ti, umax, sms, m1) || !moe_choose_plan(ms.dn, Ti, umax, sms, m2)) {
     set_error("moe: no launch configuration fits (hidden=%d, I=%d, T=%d)", ms.H, ms.I, Ti);

@@ -532,9 +532,8 @@ static int launch_backward_T(const void *y, const void *gout, const void *x, con
   const int ctas_per_sm = resident < 1 ? 1 : resident > 6 ? 6 : resident;   // 6: the register limit
   // enough warps to fill the machine, no more splits than row blocks: every warp then walks ~row_blocks / splits blocks of its
   // group, computes the group's (cos, sin) once and pays its atomics once
-  int dev = 0, sms = 0;
-  PARO_CUDA_OK(cudaGetDevice(&dev));
-  PARO_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = device_sms();
+  if (sms <= 0) { set_error("rotate_backward: no CUDA device"); return PARO_ECUDA; }
   int64_t splits = (static_cast<int64_t>(sms) * ctas_per_sm * 4 + groups - 1) / groups;
   if (splits > row_blocks) splits = row_blocks;
   if (splits < 1) splits = 1;

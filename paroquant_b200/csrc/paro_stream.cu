@@ -248,25 +248,7 @@ __device__ __forceinline__ void st_relaxed_sys_v2(uint2 *ptr, uint32_t a, uint32
   asm volatile("st.relaxed.sys.global.v2.u32 [%0], {%1, %2};" ::"l"(ptr), "r"(a), "r"(b) : "memory");
 }
 
-// ------------------------------------------------------------------ prologue: x op + rotation + B operand
-struct RotMeta {
-  uint32_t idxw[8], tw[8];
-  uint2 csw;
-  const uint8_t *meta;
-};
-
-__device__ __forceinline__ void stm_fetch_meta(const StepDesc &S, int part, int gk, int lane, RotMeta &rm) {
-  rm.meta = S.packed + S.meta_off + (static_cast<size_t>(part) * S.groups + gk) * S.meta_group_bytes;
-  rm.csw = *reinterpret_cast<const uint2 *>(rm.meta + S.krot * 256 + 8 * lane);
-  if (S.krot == 8) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      rm.idxw[r] = *reinterpret_cast<const uint32_t *>(rm.meta + r * 128 + 4 * lane);
-      rm.tw[r] = *reinterpret_cast<const uint32_t *>(rm.meta + 8 * 128 + r * 128 + 4 * lane);
-    }
-  }
-}
-
+// ------------------------------------------------------------------ prologue: the x op (rotation_tasks does the rest)
 // RMSNorm as vLLM's (fused_add_)rms_norm: T(T(h * rstd) * w)
 template <typename T> __device__ __forceinline__ uint32_t norm2(uint32_t h2, float rstd, uint32_t w2) {
   const float2 h = Traits<T>::to_float2(unpack2<T>(h2));
@@ -367,67 +349,6 @@ __device__ __forceinline__ void stm_load_x(const StepDesc &S, int M, int gk, int
         raw[m].y = norm2<T>(raw[m].y, rstd, w.y);
       }
     }
-  }
-}
-
-// B[gi][k16 step s][k half h][row m][8 k]: NR rows x 16 bytes per core-matrix column, NR * 32 bytes per step
-template <typename T, int ROWS>
-__device__ __forceinline__ void stm_write_b_rows(uint32_t xb_group, uint32_t rot, int NR, int m0, int nrows, int lane) {
-  for (int idx = lane; idx < 16 * nrows; idx += 32) {
-    const int ml = idx >> 4, s = (idx >> 1) & 7, h = idx & 1;
-    const int c0 = 16 * s + 8 * h, m = m0 + ml;
-    uint4 v;
-    if constexpr (ROWS == 1) {
-      v = lds128(rot + c0 * 2);
-    } else {
-      uint32_t e[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) e[k] = lds16(rot + (c0 + k) * (ROWS * 2) + 2 * ml);
-      v = make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
-    }
-    sts128u(xb_group + s * (NR * 32) + h * (NR * 16) + (m >> 3) * 128 + (m & 7) * 16, v);
-  }
-}
-
-template <typename T, int ROWS>
-__device__ __forceinline__ void stm_rotate_task(const StepDesc &S, int M, int NR, const RotMeta &rm, int gk, int m0, int lane, uint32_t rot,
-                                                uint32_t xb_group, uint32_t tag, uint32_t rstd_smem) {
-  uint2 raw[ROWS];
-  stm_load_x<T, ROWS>(S, M, gk, lane, raw, m0, tag, rstd_smem);
-  scale_and_stage<T, ROWS>(rot, lane, raw, rm.csw);
-  __syncwarp();
-  if (S.krot == 8) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      float c0, s0, c1, s1;
-      sincos2<T>(rm.tw[r], c0, s0, c1, s1);
-      rotate_stage<T, ROWS>(rot, rm.idxw[r], c0, s0, c1, s1);
-      __syncwarp();
-    }
-  } else {
-    const int krot = S.krot;
-    for (int r = 0; r < krot; ++r) {
-      const uint32_t iw = *reinterpret_cast<const uint32_t *>(rm.meta + r * 128 + 4 * lane);
-      const uint32_t tw = *reinterpret_cast<const uint32_t *>(rm.meta + krot * 128 + r * 128 + 4 * lane);
-      float c0, s0, c1, s1;
-      sincos2<T>(tw, c0, s0, c1, s1);
-      rotate_stage<T, ROWS>(rot, iw, c0, s0, c1, s1);
-      __syncwarp();
-    }
-  }
-  const int left = M - m0;
-  stm_write_b_rows<T, ROWS>(xb_group, rot, NR, m0, left < ROWS ? left : ROWS, lane);
-  __syncwarp();
-}
-
-// tasks t = wi, wi + nwarps, ... of ng * nq (nq row blocks per group); the first task's metadata was fetched before the waits
-template <typename T, int ROWS>
-__device__ __forceinline__ void stm_prologue(const StepDesc &S, int M, int NR, RotMeta &rm, const StepGeom &g, int ntasks, int nq, int wi,
-                                             int nwarps, int lane, uint32_t rot, uint32_t xb, uint32_t tag, uint32_t rstd_smem) {
-  for (int t = wi; t < ntasks; t += nwarps) {
-    const int gi = t / nq, rq = t - gi * nq;
-    if (t != wi) stm_fetch_meta(S, g.part, g.g_begin + gi, lane, rm);
-    stm_rotate_task<T, ROWS>(S, M, NR, rm, g.g_begin + gi, rq * ROWS, lane, rot, xb + gi * (NR * 256), tag, rstd_smem);
   }
 }
 
@@ -719,7 +640,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       const int ntasks = g.active ? g.ng * nq : 0;
       const bool mine = wi < ntasks && wi < p.rot_warps;
       RotMeta rm;
-      if (mine) stm_fetch_meta(S, g.part, g.g_begin + wi / nq, lane, rm);   // flies during the waits below
+      if (mine) fetch_meta(S.packed + S.meta_off + (static_cast<size_t>(g.part) * S.groups + g.g_begin + wi / nq) * S.meta_group_bytes, S.krot, lane, rm);   // flies during the waits below
       if (i == 0) {
         // rows [M, NR) of every group are zero padding of the MMA's N: cleared once (M is the same for every step)
         if (M < NR) {
@@ -741,13 +662,20 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
           named_bar_sync(3, 32 * nrot);
         }
         if (wi == 0) STM_TRACE(i, 2);
+        auto stage_x = [&](auto rows, int gi, int m0, uint2 csw) {
+          uint2 raw[decltype(rows)::value];
+          stm_load_x<T>(S, M, g.g_begin + gi, lane, raw, m0, tag, rstd_smem);
+          scale_and_stage<T>(rot, lane, raw, csw);
+        };
+        const uint8_t *meta = S.packed + S.meta_off;
+        const int mi0 = g.part * S.groups + g.g_begin, mg = S.meta_group_bytes, rw = p.rot_warps;
         if constexpr (MB == 1) {
-          stm_prologue<T, 1>(S, M, NR, rm, g, ntasks, nq, wi, p.rot_warps, lane, rot, xb, tag, rstd_smem);
+          rotation_tasks<T, 1, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         } else if constexpr (MB == 4) {
-          if (M == 2) stm_prologue<T, 2>(S, M, NR, rm, g, ntasks, nq, wi, p.rot_warps, lane, rot, xb, tag, rstd_smem);
-          else stm_prologue<T, 4>(S, M, NR, rm, g, ntasks, nq, wi, p.rot_warps, lane, rot, xb, tag, rstd_smem);
+          if (M == 2) rotation_tasks<T, 2, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
+          else rotation_tasks<T, 4, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         } else {
-          stm_prologue<T, 4>(S, M, NR, rm, g, ntasks, nq, wi, p.rot_warps, lane, rot, xb, tag, rstd_smem);
+          rotation_tasks<T, 4, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         }
       }
       named_bar_sync(2, 32 * kWorkers);   // B operand of this step complete
@@ -845,71 +773,13 @@ int stream_trace_read(unsigned long long *host, int max_ctas) {
 }
 
 // ------------------------------------------------------------------ host side: plan (pure, cached), carve-up, launch
-struct StmKnobs {
-  int sets, stages, force_c, no_pdl, trace, verbose, b8, inflight;
-};
-static const StmKnobs &stm_knobs() {
-  static const StmKnobs k = [] {
-    auto env = [](const char *name, int dflt) {
-      const char *v = getenv(name);
-      return v && *v ? atoi(v) : dflt;
-    };
-    StmKnobs x;
-    x.sets = kStmSets;
-    x.stages = env("PARO_DECODE_STAGES", 0);
-    x.force_c = env("PARO_DECODE_C", 0);
-    x.no_pdl = env("PARO_NO_PDL", 0);
-    x.trace = env("PARO_DECODE_TRACE", 0);
-    x.verbose = env("PARO_DECODE_VERBOSE", 0);
-    x.b8 = env("PARO_DECODE_B8", 1);
-    x.inflight = env("PARO_DECODE_INFLIGHT", 6);
-    return x;
-  }();
-  return k;
-}
-
 struct StepPlan {
   int c, T, max_slots, ng_max, max_rounds;
   int part_cta_begin[PARO_MAX_PARTS + 1];
 };
 
-// deal T members of a slice to the partitions, proportional to their 128-column blocks (largest remainder), >= 1 each
-static bool stm_deal_members(const Layout &L, int T, int *begin) {
-  int cb[PARO_MAX_PARTS], alloc[PARO_MAX_PARTS], total = 0;
-  double frac[PARO_MAX_PARTS];
-  if (T < L.n_parts) return false;
-  for (int p = 0; p < L.n_parts; ++p) {
-    cb[p] = L.part_block_begin[p + 1] - L.part_block_begin[p];
-    total += cb[p];
-  }
-  int used = 0;
-  for (int p = 0; p < L.n_parts; ++p) {
-    const double exact = static_cast<double>(T) * cb[p] / total;
-    alloc[p] = static_cast<int>(exact);
-    if (alloc[p] < 1) alloc[p] = 1;
-    frac[p] = exact - alloc[p];
-    used += alloc[p];
-  }
-  while (used < T) {
-    int best = 0;
-    for (int p = 1; p < L.n_parts; ++p)
-      if (frac[p] > frac[best]) best = p;
-    alloc[best]++; frac[best] -= 1.0; used++;
-  }
-  while (used > T) {
-    int best = -1;
-    for (int p = 0; p < L.n_parts; ++p)
-      if (alloc[p] > 1 && (best < 0 || frac[p] < frac[best])) best = p;
-    if (best < 0) return false;
-    alloc[best]--; frac[best] += 1.0; used--;
-  }
-  begin[0] = 0;
-  for (int p = 0; p < PARO_MAX_PARTS; ++p) begin[p + 1] = begin[p] + (p < L.n_parts ? alloc[p] : 0);
-  return true;
-}
-
 static int stm_rot_rows(int M) { return M == 1 ? 1 : M == 2 ? 2 : 4; }
-static int stm_b_rows(int M) { return (M <= 8 && stm_knobs().b8) ? 8 : 16; }
+static int stm_b_rows(int M) { return (M <= 8 && knobs().b8) ? 8 : 16; }
 
 // The plan of one step on `ctas` CTAs: the number of K slices c.  Pure host logic (tests drive it through
 // paro_debug_stream_plan).  Cost in "round units" (8 per dequant round): the busiest CTA's rounds, the rotation passes of
@@ -925,7 +795,7 @@ static bool stm_choose_plan(const Layout &L, int M, int sets, int ctas, int forc
     pl.c = c;
     pl.T = ctas / c;
     if (pl.T < 1) break;
-    if (!stm_deal_members(L, pl.T, pl.part_cta_begin)) continue;
+    if (!apportion(L, pl.T, pl.part_cta_begin)) continue;   // the slice's members dealt to the partitions
     pl.ng_max = (L.groups + c - 1) / c;
     const int xb_bytes = pl.ng_max * NR * 256;
     const int nst_room = (kStmSmemLimit - xb_bytes - 4 * sets * kGroup * 2 * stm_rot_rows(M) - kStmBarBytes - kStmMiscBytes - kStmDBufs * M * 1024 - 256) /
@@ -974,23 +844,9 @@ static bool stm_cached_plan(const Layout &L, int M, int sets, int ctas, StepPlan
   std::lock_guard<std::mutex> lock(mu);
   auto it = cache.find(k);
   if (it != cache.end()) { out = it->second; return true; }
-  if (!stm_choose_plan(L, M, sets, ctas, stm_knobs().force_c, out)) return false;
+  if (!stm_choose_plan(L, M, sets, ctas, knobs().force_c, out)) return false;
   cache[k] = out;
   return true;
-}
-
-static int stm_device_sms() {
-  static std::mutex mu;
-  static std::map<int, int> sms;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = sms.find(dev);
-  if (it != sms.end()) return it->second;
-  int n = 0;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
-  sms[dev] = n;
-  return n;
 }
 
 // test hook: out[0..4] = c, T, max_slots, ng_max, max_rounds; out[5..13] = part_cta_begin
@@ -1027,13 +883,13 @@ bool stream_supported(const Layout &L, int64_t M) { return M >= 1 && M <= 16 && 
 // never touched by the large-M path, which keeps its scratch behind them)
 size_t stream_sync_bytes(const Layout &) { return kStmSyncBytes; }
 size_t stream_workspace_bytes(const Layout &L, int64_t max_m) {
-  const int sms = stm_device_sms();
-  const int ctas = sms > 0 ? sms : 132;
+  const int sms = device_sms();
+  const int ctas = sms > 0 ? sms : 132;   // no device: size for an H100
   size_t need = kStmSyncBytes;
   const int top = max_m < 16 ? static_cast<int>(max_m) : 16;
   for (int M = 1; M <= top; ++M) {
     StepPlan pl;
-    if (!stm_cached_plan(L, M, stm_knobs().sets, ctas, pl)) continue;
+    if (!stm_cached_plan(L, M, kStmSets, ctas, pl)) continue;
     const StepWs w = stm_step_ws(L, pl, M, kStmSyncBytes, false);
     if (w.end > need) need = w.end;
   }
@@ -1043,7 +899,7 @@ size_t stream_workspace_bytes(const Layout &L, int64_t max_m) {
 template <typename T, int SETS, int MB>
 static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream) {
   auto kern = stream_kernel<T, SETS, MB>;
-  const StmKnobs &kn = stm_knobs();
+  const Knobs &kn = knobs();
   const int M = p.M;
   p.nrows_b = stm_b_rows(M);
   p.rot_bytes = kGroup * 2 * stm_rot_rows(M);
@@ -1085,32 +941,21 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
               p.steps[i].N, M, p.steps[i].c, p.steps[i].T, p.steps[i].max_slots, p.steps[i].x_op, p.steps[i].epi_op, p.steps[i].x_ll ? 1 : 0);
     fprintf(stderr, "[paro stream] %d CTAs, %d stages, B rows %d, rot warps %d, smem %d\n", ctas, p.nstages, p.nrows_b, p.rot_warps, smem_total);
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(32 * (4 * SETS + 5));
-  cfg.dynamicSmemBytes = smem_total;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  int na = 0;
-  if (!kn.no_pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[2];
+  launch_config(cfg, attr, ctas, 32 * (4 * SETS + 5), smem_total, stream, 0, !kn.no_pdl);
   PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
   note_launches(1);
   return PARO_OK;
 }
 
 size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) {
-  const int sms = stm_device_sms();
-  const int ctas = sms > 0 ? sms : 132;
+  const int sms = device_sms();
+  const int ctas = sms > 0 ? sms : 132;   // no device: size for an H100
   size_t off = kStmSyncBytes;
   for (int i = 0; i < n; ++i) {
     StepPlan pl;
-    if (!stm_cached_plan(steps[i].L, static_cast<int>(M), stm_knobs().sets, ctas, pl)) return 0;
+    if (!stm_cached_plan(steps[i].L, static_cast<int>(M), kStmSets, ctas, pl)) return 0;
     const bool consumed = i + 1 < n && !steps[i + 1].x;
     off = stm_step_ws(steps[i].L, pl, static_cast<int>(M), off, consumed).end;
   }
@@ -1118,8 +963,8 @@ size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) {
 }
 
 int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const StmKnobs &kn = stm_knobs();
-  const int sms = stm_device_sms();
+  const Knobs &kn = knobs();
+  const int sms = device_sms();
   if (sms <= 0) { set_error("decode: no CUDA device"); return PARO_ECUDA; }
   StreamParams p;
   memset(&p, 0, sizeof(p));
@@ -1136,7 +981,7 @@ int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, siz
     const Layout &L = h.L;
     if (L.dtype != dtype) { set_error("chain: every step must use the same activation dtype"); return PARO_EINVAL; }
     StepPlan pl;
-    if (!stm_cached_plan(L, p.M, kn.sets, sms, pl)) {
+    if (!stm_cached_plan(L, p.M, kStmSets, sms, pl)) {
       set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, p.M);
       return PARO_EUNSUPPORTED;
     }

@@ -1,7 +1,10 @@
-// Device helpers shared by the tensor-core kernels (paro_decode.cu, paro_gemm.cu):
-// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T A-fragment dequant
-// and the in-warp pairwise rotation (rounding points of /root/reference/paroquant/kernels/cuda/rotation.cuh:91-173).
+// Device helpers shared by the tensor-core kernels (paro_decode.cu, paro_stream.cu, paro_moe.cu, paro_gemm.cu):
+// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T A-fragment dequant,
+// the in-warp pairwise rotation (rounding points of /root/reference/paroquant/kernels/cuda/rotation.cuh:91-173) and the
+// small-M kernels' rotation prologue built from it (rotation_tasks).
 #pragma once
+#include <type_traits>
+
 #include "paro_common.cuh"
 #include "paro_layout.h"
 
@@ -279,17 +282,6 @@ __device__ __forceinline__ void rotate_stage(uint32_t rot, uint32_t idxw, float 
   }
 }
 
-// this lane's 4 channels of the group for all rows: raw x (no dependence on the rotation metadata)
-template <typename T, int ROWS, typename P>
-__device__ __forceinline__ void load_x(const P &p, int gk, int lane, uint2 (&raw)[ROWS], int m0 = 0) {
-  const T *xg = static_cast<const T *>(p.x) + gk * kGroup + 4 * lane;   // (p.x already points at the CTA's partition when pre-rotated)
-#pragma unroll
-  for (int m = 0; m < ROWS; ++m) {
-    raw[m] = make_uint2(0u, 0u);
-    if (m0 + m < p.M) raw[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * p.K));
-  }
-}
-
 // multiply by the channel scales in T (one rounding, rotation.cuh:112-113), lay out channel-major in `rot`
 template <typename T, int ROWS>
 __device__ __forceinline__ void scale_and_stage(uint32_t rot, int lane, const uint2 (&raw)[ROWS], uint2 csw) {
@@ -331,6 +323,89 @@ __device__ __forceinline__ void sincos2(uint32_t theta_pair_bits, float &c0, flo
   const float2 th = Traits<T>::to_float2(unpack2<T>(theta_pair_bits));
   __sincosf(th.x, &s0, &c0);
   __sincosf(th.y, &s1, &c1);
+}
+
+// ------------------------------------------------------------------ rotation prologue of the small-M kernels
+// One group's rotation metadata (paro_layout.h) as this lane uses it: its 4 channel scales and, for krot = 8, its pair-index
+// and theta words of every stage -- fetched with the scales, so they fly during whatever the kernel waits for before x.
+struct RotMeta {
+  uint32_t idxw[8], tw[8];
+  uint2 csw;
+  const uint8_t *meta;
+};
+
+template <bool REGS8 = true>
+__device__ __forceinline__ void fetch_meta(const uint8_t *meta, int krot, int lane, RotMeta &rm) {
+  rm.meta = meta;
+  rm.csw = *reinterpret_cast<const uint2 *>(meta + krot * 256 + 8 * lane);
+  if (REGS8 && krot == 8) {
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      rm.idxw[r] = *reinterpret_cast<const uint32_t *>(meta + r * 128 + 4 * lane);
+      rm.tw[r] = *reinterpret_cast<const uint32_t *>(meta + 8 * 128 + r * 128 + 4 * lane);
+    }
+  }
+}
+
+// rows m0 .. m0 + nrows - 1 of a rotation tile into the group's B operand, B[k16 step s][k half h][row m][8 k]: NR rows x 16 bytes
+// per core-matrix column, NR * 32 bytes per step (NR = 8 or 16; a literal 16 folds into the addressing)
+template <typename T, int ROWS>
+__device__ __forceinline__ void write_b_rows(uint32_t xb_group, uint32_t rot, int NR, int m0, int nrows, int lane) {
+  for (int idx = lane; idx < 16 * nrows; idx += 32) {
+    const int ml = idx >> 4, s = (idx >> 1) & 7, h = idx & 1;
+    const int c0 = 16 * s + 8 * h, m = m0 + ml;
+    uint4 v;
+    if constexpr (ROWS == 1) {
+      v = lds128(rot + c0 * 2);
+    } else {
+      uint32_t e[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) e[k] = lds16(rot + (c0 + k) * (ROWS * 2) + 2 * ml);
+      v = make_uint4(e[0] | (e[1] << 16), e[2] | (e[3] << 16), e[4] | (e[5] << 16), e[6] | (e[7] << 16));
+    }
+    sts128u(xb_group + s * (NR * 32) + h * (NR * 16) + (m >> 3) * 128 + (m & 7) * 16, v);
+  }
+}
+
+// A warp's rotation tasks t = wi, wi + nwarps, ... < ntasks: task t is group gi = t / nq of the warp's groups (metadata block
+// mi0 + gi of `meta`, meta_group_bytes each) x token rows m0 = ROWS * (t % nq) .. of `rows`.  The kernel's x loader
+// stage_x(ROWS tag, gi, m0, csw) loads this lane's 4 channels of those rows after the kernel's x op and stages them in `rot`
+// (scale_and_stage); here they go through the krot stages into group gi's B operand, xb + gi * NR * 256.  rm holds the first
+// task's metadata, which the caller fetched ahead of its waits (fetch_meta<REGS8>).  REGS8: krot = 8 takes its stage words from
+// rm's registers; without it every krot reads them in the stage loop (the MoE kernel: its tasks follow no wait to hide them
+// behind, and the register path costs it ~15 registers and ~80 % more SASS).
+template <typename T, int ROWS, bool REGS8, typename StageX>
+__device__ __forceinline__ void rotation_tasks(RotMeta &rm, const uint8_t *meta, int meta_group_bytes, int krot, int mi0, int ntasks, int nq,
+                                               int rows, int wi, int nwarps, int lane, uint32_t rot, uint32_t xb, int NR, StageX stage_x) {
+  for (int t = wi; t < ntasks; t += nwarps) {
+    const int gi = t / nq, m0 = (t - gi * nq) * ROWS;
+    if (t != wi) fetch_meta<REGS8>(meta + static_cast<size_t>(mi0 + gi) * meta_group_bytes, krot, lane, rm);
+    stage_x(std::integral_constant<int, ROWS>{}, gi, m0, rm.csw);
+    __syncwarp();
+    if (REGS8 && krot == 8) {
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        // (keeping all 32 coefficients live across griddepcontrol.wait was tried: it spills at 80 registers and the
+        // stages get slower than with the MUFU work inline)
+        float c0, s0, c1, s1;
+        sincos2<T>(rm.tw[r], c0, s0, c1, s1);
+        rotate_stage<T, ROWS>(rot, rm.idxw[r], c0, s0, c1, s1);
+        __syncwarp();
+      }
+    } else {
+      for (int r = 0; r < krot; ++r) {
+        const uint32_t iw = *reinterpret_cast<const uint32_t *>(rm.meta + r * 128 + 4 * lane);
+        const uint32_t tw = *reinterpret_cast<const uint32_t *>(rm.meta + krot * 128 + r * 128 + 4 * lane);
+        float c0, s0, c1, s1;
+        sincos2<T>(tw, c0, s0, c1, s1);
+        rotate_stage<T, ROWS>(rot, iw, c0, s0, c1, s1);
+        __syncwarp();
+      }
+    }
+    const int left = rows - m0;
+    write_b_rows<T, ROWS>(xb + gi * (NR * 256), rot, NR, m0, left < ROWS ? left : ROWS, lane);
+    __syncwarp();
+  }
 }
 
 }  // namespace paro

@@ -39,7 +39,7 @@ for i in range(1, 9):
         print(f"  {names[i]:28s} +{np.median(d):9.0f} cyc median  (min {d.min():8.0f}  max {d.max():8.0f})   cumulative median {np.median(cur[ok]):9.0f}")
     prev = np.where(ok, cur, prev)
 if t[:, 9].max() > 0:
-    print(f"  (one-CTA-per-SM kernel) x loaded+scaled at {np.median(t[:, 0]):.0f}, rotation stages done at {np.median(t[:, 9]):.0f} (cumulative cycles, median)")
+    print(f"  (one-CTA-per-SM kernel) warp 0's last rotation task: x loaded+scaled at {np.median(t[:, 0]):.0f}, rotated rows written at {np.median(t[:, 9]):.0f} (cumulative cycles, median)")
 g0, g1 = t[:, 10].astype(np.int64), t[:, 11].astype(np.int64)
 print(f"  globaltimer: first entry -> last exit {(g1.max() - g0.min())} ns; entry spread {g0.max() - g0.min()} ns; per-CTA duration median {np.median(g1 - g0):.0f} ns")
 
