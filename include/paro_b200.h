@@ -24,7 +24,7 @@
  *                            paroquant/inference/backends/transformers/modules.py:57-71
  *   paro_last_error        TORCH_CHECK messages of rotation.cu:66,92,108,114,123
  *   paro_moe_forward       RotateSwitchGLU  paroquant/inference/backends/mlx/modules.py:159-212 on the
- *                            expert format of paroquant/cli/convert.py:281-406
+ *   paro_moe_grouped_forward expert format of paroquant/cli/convert.py:281-406 (decode batches / any batch)
  *
  * Return value of every int function: 0 on success, a PARO_E* code otherwise; the message is
  * available from paro_last_error() on the same thread.
@@ -232,6 +232,35 @@ int paro_moe_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_
  * coverage violations over U = 1..U_max (a (expert slot, group) round of a block owned other than exactly once, or rank 0
  * reading a receive slot no rank wrote in that wave).                                                                  */
 int paro_debug_moe_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out);
+
+/* ---- MoE expert block for any batch: the routed experts as grouped INT4 wgmma GEMMs, routing read on the device ----------
+ * Same descriptor, semantics, alignments and checks as paro_moe_forward, for batches the decode kernel does not take (prefill,
+ * or more than 16 sequences in flight).  Six launches (paroquant_b200/csrc/paro_moe_grouped.cu): the routing table (entries
+ * sorted by expert, each expert's run padded to whole tiles of NT rows), the gate_up pre-pass (x gathered through the table,
+ * rotated once per entry), the grouped gate_up GEMM (scattered to h), the down pre-pass (SiLU * up of h, rotated), the grouped
+ * down GEMM (into the workspace) and the per-token combine.  No host synchronisation, no allocation; the plan depends on
+ * (T, top_k, n_experts) only, so a captured CUDA graph stays valid while the ids / weights in its buffers change.  Every
+ * h[t, s] and y_s row is computed independently of the tiling: permuting tokens or slots permutes h and y bit for bit.
+ * paro_last_launch_count() reports 6.                                                                                     */
+#define PARO_MOE_GROUPED_MAX_ENTRIES 65536   /* T * top_k                                                                   */
+#define PARO_MOE_GROUPED_MAX_EXPERTS 1024
+
+/* Workspace bytes for paro_moe_grouped_forward (0 on an invalid descriptor or batch): the routing table, the rotated operand
+ * of both GEMMs (tiles_max x NT rows of max(hidden, I) elements) and the y_s rows (T x top_k x hidden elements).           */
+size_t paro_moe_grouped_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t top_k);
+
+/* Run the expert block for T tokens with top_k slots each; arguments as paro_moe_forward, workspace 256-byte aligned.
+ * 1 <= top_k <= 16, T >= 1, T * top_k <= PARO_MOE_GROUPED_MAX_ENTRIES and n_experts <= PARO_MOE_GROUPED_MAX_EXPERTS;
+ * otherwise PARO_EUNSUPPORTED.  A workspace below paro_moe_grouped_workspace_bytes gives PARO_EWORKSPACE.              */
+int paro_moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_ids, const float *topk_weights,
+                             int64_t T, int32_t top_k, void *h, void *y, void *workspace, size_t workspace_bytes,
+                             paro_stream_t stream);
+
+/* Test hook (host only): the plan of paro_moe_grouped_forward.  out[0] = NT (rows per tile: 32, 64 or 128), out[1] = tiles_max
+ * = floor(T * top_k / NT) + min(n_experts, T * top_k), out[2..7] = grid of each launch (route, gate_up pre-pass, gate_up GEMM,
+ * down pre-pass, down GEMM, combine), out[8..11] = workspace bytes / 256 of the routing table, the operand, the y_s rows and
+ * in total.  The plan does not depend on the SM count; `sms` must be >= 1.                                                */
+int paro_debug_moe_grouped_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out);
 
 /* Debug / test aid: dequantise the prepacked weights back to a dense [K, N] matrix of
  * shape->dtype (the exact operand the GEMM consumes).                                    */

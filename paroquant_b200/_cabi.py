@@ -119,6 +119,12 @@ def lib() -> ctypes.CDLL:
         L.paro_moe_forward.argtypes = [moe, vp, vp, vp, i64, i32, vp, vp, vp, sz, vp]
         L.paro_debug_moe_plan.restype = ctypes.c_int
         L.paro_debug_moe_plan.argtypes = [moe, i64, i32, i32, ctypes.POINTER(ctypes.c_int32)]
+        L.paro_moe_grouped_workspace_bytes.restype = sz
+        L.paro_moe_grouped_workspace_bytes.argtypes = [moe, i64, i32]
+        L.paro_moe_grouped_forward.restype = ctypes.c_int
+        L.paro_moe_grouped_forward.argtypes = [moe, vp, vp, vp, i64, i32, vp, vp, vp, sz, vp]
+        L.paro_debug_moe_grouped_plan.restype = ctypes.c_int
+        L.paro_debug_moe_grouped_plan.argtypes = [moe, i64, i32, i32, ctypes.POINTER(ctypes.c_int32)]
         if L.paro_abi_version() != ABI_VERSION:
             raise ImportError("libparo_b200.so ABI version mismatch")
         _lib = L
@@ -130,6 +136,7 @@ EXPORTED_SYMBOLS = (
     "paro_prepack", "paro_workspace_bytes", "paro_linear_forward", "paro_unpack_dense", "paro_debug_trace", "paro_debug_decode_plan",
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
     "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan", "paro_debug_silu_mul",
+    "paro_moe_grouped_workspace_bytes", "paro_moe_grouped_forward", "paro_debug_moe_grouped_plan",
 )
 
 
@@ -362,27 +369,51 @@ def moe_forward(desc: ParoMoEDesc, x: torch.Tensor, topk_ids: torch.Tensor, topk
                 workspace: torch.Tensor) -> None:
     """paro_moe_forward on the current stream of x's device: x [T, hidden], topk_ids [T, k] int32, topk_weights [T, k] fp32,
     h [T, k, 2I] and y [T, hidden] of the experts' dtype, all contiguous on one CUDA device."""
+    _moe_call("moe_forward", lib().paro_moe_forward, desc, x, topk_ids, topk_weights, h, y, workspace)
+
+
+def moe_grouped_forward(desc: ParoMoEDesc, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor, h: torch.Tensor,
+                        y: torch.Tensor, workspace: torch.Tensor) -> None:
+    """paro_moe_grouped_forward (any T) with the arguments of moe_forward; the workspace holds moe_grouped_workspace_bytes."""
+    _moe_call("moe_grouped_forward", lib().paro_moe_grouped_forward, desc, x, topk_ids, topk_weights, h, y, workspace)
+
+
+def moe_grouped_workspace_bytes(desc: ParoMoEDesc, T: int, top_k: int) -> int:
+    nb = lib().paro_moe_grouped_workspace_bytes(ctypes.byref(desc), T, top_k)
+    if nb == 0:
+        raise RuntimeError(f"moe_grouped: {lib().paro_last_error().decode()}")
+    return nb
+
+
+def debug_moe_grouped_plan(desc: ParoMoEDesc, T: int, top_k: int, sms: int) -> list[int]:
+    """[NT, tiles_max, six launch grids, workspace regions / 256 (table, operand, y_s, total)] (include/paro_b200.h)."""
+    out = (ctypes.c_int32 * 12)()
+    _check(lib().paro_debug_moe_grouped_plan(ctypes.byref(desc), T, top_k, sms, out), "debug_moe_grouped_plan")
+    return list(out)
+
+
+def _moe_call(what: str, fn, desc: ParoMoEDesc, x, topk_ids, topk_weights, h, y, workspace) -> None:
     dt = _CODE_DTYPE[desc.gate_up.contents.dtype]
     H, I2 = desc.gate_up.contents.in_features, desc.gate_up.contents.out_features
     if topk_ids.dtype != torch.int32 or topk_weights.dtype != torch.float32:
-        raise RuntimeError(f"moe_forward: topk_ids must be int32 and topk_weights float32, got {topk_ids.dtype} / {topk_weights.dtype}")
+        raise RuntimeError(f"{what}: topk_ids must be int32 and topk_weights float32, got {topk_ids.dtype} / {topk_weights.dtype}")
     for name, t in (("x", x), ("h", h), ("y", y)):
         if t.dtype != dt:
-            raise RuntimeError(f"moe_forward: {name} must be {dt}, got {t.dtype}")
+            raise RuntimeError(f"{what}: {name} must be {dt}, got {t.dtype}")
     dev = _need_cuda(x, topk_ids, topk_weights, h, y, workspace)
     if topk_ids.dim() != 2 or tuple(topk_weights.shape) != tuple(topk_ids.shape):
-        raise RuntimeError("moe_forward: topk_ids and topk_weights must both be [T, k]")
+        raise RuntimeError(f"{what}: topk_ids and topk_weights must both be [T, k]")
     T, k = topk_ids.shape
     want = {"x": ((T, H), x), "h": ((T, k, I2), h), "y": ((T, H), y)}
     for name, (shp, t) in want.items():
         if tuple(t.shape) != shp:
-            raise RuntimeError(f"moe_forward: {name} must be {shp}, got {tuple(t.shape)}")
+            raise RuntimeError(f"{what}: {name} must be {shp}, got {tuple(t.shape)}")
     if not all(t.is_contiguous() for t in (x, topk_ids, topk_weights, h, y)):
-        raise RuntimeError("moe_forward: all tensors must be contiguous")
+        raise RuntimeError(f"{what}: all tensors must be contiguous")
     with torch.cuda.device(dev):
-        rc = lib().paro_moe_forward(ctypes.byref(desc), x.data_ptr(), topk_ids.data_ptr(), topk_weights.data_ptr(), T, k, h.data_ptr(),
-                                    y.data_ptr(), workspace.data_ptr(), workspace.numel(), _stream(dev))
-    _check(rc, "moe_forward")
+        rc = fn(ctypes.byref(desc), x.data_ptr(), topk_ids.data_ptr(), topk_weights.data_ptr(), T, k, h.data_ptr(), y.data_ptr(),
+                workspace.data_ptr(), workspace.numel(), _stream(dev))
+    _check(rc, what)
 
 
 def debug_moe_plan(desc: ParoMoEDesc, T: int, top_k: int, sms: int) -> list[int]:

@@ -57,6 +57,10 @@ int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const
                 void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, int32_t *out);
 int moe_debug_silu_mul(int dtype, const void *gate_up, void *act, int64_t M, int I, cudaStream_t stream);
+size_t moe_grouped_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);
+int moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const float *wts, int64_t T, int32_t k, void *h, void *y,
+                        void *workspace, size_t workspace_bytes, cudaStream_t stream);
+int moe_grouped_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t *out);
 
 const Knobs &knobs() {
   static const Knobs k = [] {
@@ -336,6 +340,19 @@ int paro_moe_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_
 int paro_debug_moe_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out) {
   if (!out || sms < 1) { set_error("debug_moe_plan: bad arguments"); return PARO_EINVAL; }
   return moe_debug_plan(d, T, top_k, sms, out);
+}
+
+size_t paro_moe_grouped_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t top_k) { return moe_grouped_workspace_bytes(d, T, top_k); }
+
+int paro_moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *topk_ids, const float *topk_weights, int64_t T, int32_t top_k,
+                             void *h, void *y, void *workspace, size_t workspace_bytes, paro_stream_t stream) {
+  g_launches = 0;
+  return moe_grouped_forward(d, x, topk_ids, topk_weights, T, top_k, h, y, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int paro_debug_moe_grouped_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out) {
+  if (!out || sms < 1) { set_error("debug_moe_grouped_plan: bad arguments"); return PARO_EINVAL; }
+  return moe_grouped_debug_plan(d, T, top_k, out);
 }
 
 int paro_debug_stream_trace(unsigned long long *host_out, int32_t max_ctas) {

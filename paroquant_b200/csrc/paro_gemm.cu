@@ -14,6 +14,10 @@
 // Warpgroup 0: warp 0 TMA producer of the weight records (one 8576-byte record per round), warp 1 TMA producer of the
 // x_rot stages.  Warpgroups 1 and 2: consumers of output columns 0-63 / 64-127 of the block; a consumer dequantises
 // round r + 1 while the wgmmas of round r run (two register sets of A fragments).
+//
+// The same kernel serves the MoE block's grouped GEMMs (paro_moe_grouped.cu) through its tile source: there a token block is a
+// tile slot of the routing table -- NT sorted (token, slot) rows of one expert -- the weights are that expert's, and the
+// epilogue scatters each row to its (token, slot) output row.
 #include "paro_tc_common.cuh"
 
 namespace paro {
@@ -40,6 +44,20 @@ struct GemmParams {
   long long rec_off, xr_part_stride;
 };
 
+// Tile source of a linear: token block tb is rows tb * NT .. tb * NT + NT - 1 of x and y, the weights are p.packed.
+struct DenseTiles {
+  static constexpr bool kGrouped = false;
+};
+// Tile source of a MoE block's grouped GEMM: tile slot tb is positions tb * NT .. of the routing table, all of one expert
+// (paro_moe_grouped.cu writes the table on the device).  Slots from *live_tiles on are empty and exit at once.
+struct GroupedTiles {
+  static constexpr bool kGrouped = true;
+  const int32_t *rows;          // [slots * NT]: output row (token * top_k + slot) of each position, -1 for padding
+  const int32_t *tile_expert;   // [slots]
+  const int32_t *live_tiles;
+  long long expert_stride;      // bytes from one expert's packed buffer to the next
+};
+
 // the A fragments of one round (8 k16 steps x 4 registers) for this warp's 16-row tile: two 128-bit loads per lane
 template <typename T>
 __device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32_t zero_off, int tile, int lane, uint32_t (&a)[32]) {
@@ -53,8 +71,8 @@ __device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32
   d.frag(w1.x, a + 16); d.frag(w1.y, a + 20); d.frag(w1.z, a + 24); d.frag(w1.w, a + 28);
 }
 
-template <typename T, int NT>
-__global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmParams p) {
+template <typename T, int NT, typename Tiles>
+__global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmParams p, const Tiles tiles) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t smem0 = smem_u32(smem);
@@ -68,6 +86,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
   while (block >= p.part_block_begin[part + 1]) ++part;
   const int n0 = p.part_col_begin[part] + (block - p.part_block_begin[part]) * kBlockN, n_end = p.part_col_begin[part + 1];
   const int rounds = p.groups;
+  const uint8_t *packed = p.packed;
+  if constexpr (Tiles::kGrouped) {
+    pdl_wait();   // the routing table (written two launches back) names the tile's expert
+    if (tb >= *tiles.live_tiles) return;
+    packed += tiles.tile_expert[tb] * tiles.expert_stride;
+  }
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kWStages; ++s) { mbar_init(bar_wfull + 8 * s, 1); mbar_init(bar_wempty + 8 * s, 4 * kGemmConsumers); }
@@ -81,7 +105,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     // all token blocks, so the records stay under the normal L2 policy (no evict-first here)
     if (lane == 0) {
       const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
-      const uint8_t *rec = p.packed + p.rec_off + static_cast<size_t>(block) * p.groups * rec_bytes;
+      const uint8_t *rec = packed + p.rec_off + static_cast<size_t>(block) * p.groups * rec_bytes;
       for (int r = 0; r < rounds; ++r) {
         const int ws = r % kWStages, wit = r / kWStages;
         if (wit > 0) mbar_wait(bar_wempty + 8 * ws, (wit - 1) & 1);
@@ -182,7 +206,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int64_t m = static_cast<int64_t>(tb) * NT + 8 * j + 2 * t + e;
-          if (m < p.M) {
+          if constexpr (Tiles::kGrouped) {
+            const int row = tiles.rows[m];
+            if (row >= 0) yout[static_cast<int64_t>(row) * p.N + n] = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
+          } else if (m < p.M) {
             T v = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
             if (has_bias) v = Traits<T>::from_float(Traits<T>::to_float(v) + bias_f);
             yout[m * p.N + n] = v;
@@ -229,24 +256,36 @@ size_t gemm_workspace_bytes(const Layout &L, int64_t max_m) {
   return static_cast<size_t>(L.n_parts) * m_pad * L.K * 2;   // x_rot per partition, B-operand tile order
 }
 
-template <typename T, int NT>
-static int launch_gemm(const GemmParams &p, cudaStream_t stream) {
-  auto kern = wg_gemm_kernel<T, NT>;
+template <typename T, int NT, typename Tiles>
+static int launch_gemm(const GemmParams &p, const Tiles &tiles, cudaStream_t stream) {
+  auto kern = wg_gemm_kernel<T, NT, Tiles>;
   const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256;
   PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, p.n_blocks * p.tok_blocks, kGemmThreads, smem, stream, 0, true);   // PDL: prologue + first weight stages overlap the pre-pass
-  PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
+  PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p, tiles));
   note_launches(1);
   return PARO_OK;
 }
 
-template <typename T>
-static int launch_gemm_nt(const GemmParams &p, cudaStream_t stream) {
-  if (p.NT == 128) return launch_gemm<T, 128>(p, stream);
-  if (p.NT == 64) return launch_gemm<T, 64>(p, stream);
-  return launch_gemm<T, 32>(p, stream);
+template <typename T, typename Tiles = DenseTiles>
+static int launch_gemm_nt(const GemmParams &p, cudaStream_t stream, const Tiles &tiles = Tiles{}) {
+  if (p.NT == 128) return launch_gemm<T, 128>(p, tiles, stream);
+  if (p.NT == 64) return launch_gemm<T, 64>(p, tiles, stream);
+  return launch_gemm<T, 32>(p, tiles, stream);
+}
+
+static void fill_weights(GemmParams &p, const Layout &L) {
+  p.K = L.K; p.N = L.N;
+  p.n_blocks = L.blocks_total;
+  p.n_parts = L.n_parts; p.groups = L.groups;
+  p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2;
+  for (int i = 0; i <= PARO_MAX_PARTS; ++i) {
+    p.part_col_begin[i] = L.part_col_begin[i];
+    p.part_block_begin[i] = L.part_block_begin[i];
+  }
+  p.rec_off = static_cast<long long>(L.rec_off);
 }
 
 int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
@@ -272,19 +311,31 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
   p.xr = xr_base;
   p.y = y;
   p.bias = bias;
-  p.M = static_cast<int>(M); p.K = L.K; p.N = L.N; p.NT = NT;
-  p.n_blocks = L.blocks_total;
+  fill_weights(p, L);
+  p.M = static_cast<int>(M); p.NT = NT;
   p.tok_blocks = static_cast<int>(m_pad / NT);
-  p.n_parts = L.n_parts; p.groups = L.groups;
-  p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2;
-  for (int i = 0; i <= PARO_MAX_PARTS; ++i) {
-    p.part_col_begin[i] = L.part_col_begin[i];
-    p.part_block_begin[i] = L.part_block_begin[i];
-  }
-  p.rec_off = static_cast<long long>(L.rec_off);
   p.xr_part_stride = static_cast<long long>(m_pad) * L.K * 2;
   if (s.dtype == PARO_BF16) return launch_gemm_nt<__nv_bfloat16>(p, stream);
   return launch_gemm_nt<__half>(p, stream);
+}
+
+// One grouped GEMM of a MoE block (paro_moe_grouped.cu): y[rows[m], :] = x_rot[m, :] . W[expert of m's tile] for every live tile
+// slot.  `xr` holds `slots` tiles of NT rows in B-operand order, written by the pre-pass; every partition of L reads it (a MoE
+// block's gate and up share one rotation).  `packed` is expert 0's buffer, expert e's lies `expert_stride` bytes further on.
+int gemm_grouped_launch(const Layout &L, const void *packed, long long expert_stride, const void *xr, void *y, int NT, int slots,
+                        const int32_t *rows, const int32_t *tile_expert, const int32_t *live_tiles, int dtype, cudaStream_t stream) {
+  GemmParams p = {};
+  fill_weights(p, L);
+  p.packed = static_cast<const uint8_t *>(packed);
+  p.xr = static_cast<const uint8_t *>(xr);
+  p.y = y;
+  p.bias = nullptr;
+  p.M = slots * NT; p.NT = NT;
+  p.tok_blocks = slots;
+  p.xr_part_stride = 0;
+  const GroupedTiles tiles = {rows, tile_expert, live_tiles, expert_stride};
+  if (dtype == PARO_BF16) return launch_gemm_nt<__nv_bfloat16>(p, stream, tiles);
+  return launch_gemm_nt<__half>(p, stream, tiles);
 }
 
 }  // namespace paro

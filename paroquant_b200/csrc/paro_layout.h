@@ -156,4 +156,9 @@ inline bool apportion(const Layout &L, int count, int *begin) {
   return true;
 }
 
+// A MoE block's two layouts (every expert's gate_up and down), the expert count, intermediate and hidden size.  moe_check_desc
+// (paro_moe.cu) validates a paro_moe_desc into it for both MoE paths, with the error message set on failure.
+struct MoeShapes { Layout gu, dn; int E, I, H; };
+int moe_check_desc(const paro_moe_desc *d, MoeShapes &ms);
+
 }  // namespace paro

@@ -348,9 +348,7 @@ static bool moe_choose_plan(const Layout &L, int T, int umax, int sms, MoePlan &
   return best_cost >= 0;
 }
 
-struct MoeShapes { Layout gu, dn; int E, I, H; };
-
-static int moe_check(const paro_moe_desc *d, int64_t T, int32_t k, MoeShapes &ms) {
+int moe_check_desc(const paro_moe_desc *d, MoeShapes &ms) {
   const char *why = "";
   if (!d || !d->gate_up || !d->down) { set_error("moe: null descriptor or shape"); return PARO_EINVAL; }
   if (!make_layout(*d->gate_up, ms.gu, &why)) { set_error("moe: gate_up: %s", why); return PARO_EINVAL; }
@@ -372,6 +370,12 @@ static int moe_check(const paro_moe_desc *d, int64_t T, int32_t k, MoeShapes &ms
               d->gate_up_stride, d->down_stride);
     return PARO_EINVAL;
   }
+  return PARO_OK;
+}
+
+static int moe_check(const paro_moe_desc *d, int64_t T, int32_t k, MoeShapes &ms) {
+  const int rc = moe_check_desc(d, ms);
+  if (rc) return rc;
   if (T < 1 || T > 16 || k < 1 || k > 16 || T * k > kMoeMaxEntries) {
     set_error("moe: 1 <= T <= 16, 1 <= top_k <= 16 and T * top_k <= %d supported, got T = %lld, top_k = %d", kMoeMaxEntries,
               static_cast<long long>(T), k);

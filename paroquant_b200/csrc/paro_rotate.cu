@@ -12,6 +12,7 @@
 // loads and two 128-bit stores for all RB rows at once.  The 16-byte slot of channel c is
 // c ^ ((c >> 3) & 7), which makes the coalesced transpose-in / transpose-out conflict free.
 #include "paro_common.cuh"
+#include "paro_tc_common.cuh"   // silu_mul2: the MoE down pre-pass
 
 namespace paro {
 
@@ -214,12 +215,57 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
 
 // ------------------------------------------------------------------ pre-pass of the tensor-core kernels (paro_decode.cu from 5 rows, paro_gemm.cu)
 // ONE launch for all partitions of a merged linear: warp = (partition, group, block of 8 rows); output in the B-operand order
-// of the consumer (tiles of nt tokens, rows >= M zero).  Same arithmetic as rotate_kernel; what differs is latency: the pair
+// of the consumer (tiles of nt tokens, padding rows zero).  Same arithmetic as rotate_kernel; what differs is latency: the pair
 // indices and angles of all (<= 8 at a time) rotations are fetched up front, so the launch costs one global-load round trip
 // instead of one per stage (rotate_kernel at 16 rows: ~7 us, almost all of it eight dependent L2 / DRAM latencies).
+//
+// A row source says what feeds output row m: `skip(row0)` -- the block of 8 rows from row0 on is never read, leave it;
+// `padding_block(row0)` -- all 8 rows are padding, store zeros; `valid(m)` -- row m has an input (else it is a zero row);
+// `load(m, k)` -- channels k .. k + 3 of row m's input, before the channel scale.
+
+// a linear's activations x [M, K]; rows >= M are padding
 template <typename T>
-__global__ void __launch_bounds__(128) rotate_small_kernel(const T *__restrict__ x, T *__restrict__ out, const uint8_t *__restrict__ raw_base,
-                                                           long long raw_part_bytes, long long out_part_elems, int M, int M_store, int nt, int K,
+struct DenseRows {
+  const T *x;
+  int M, K;
+  __device__ bool skip(int) const { return false; }
+  __device__ bool padding_block(int row0) const { return row0 >= M; }
+  __device__ bool valid(int m) const { return m < M; }
+  __device__ uint2 load(int m, int k) const { return *reinterpret_cast<const uint2 *>(x + static_cast<int64_t>(m) * K + k); }
+};
+
+// The MoE grouped pre-passes (paro_moe_grouped.cu): output row m is routing entry rows[m] = token * top_k + slot, -1 for padding.
+// Padding runs from an expert's last entry to the end of its tile, so a block of 8 rows starting on padding is all padding.
+// Rows from live_tiles * nt on belong to no tile the GEMM runs.
+struct RoutedRows {
+  const int32_t *rows, *live_tiles;
+  int nt;
+  __device__ bool skip(int row0) const { return row0 >= *live_tiles * nt; }
+  __device__ bool padding_block(int row0) const { return rows[row0] < 0; }
+  __device__ bool valid(int m) const { return rows[m] >= 0; }
+};
+// gate_up: x [T, K], entry e reads token e / top_k
+template <typename T>
+struct GatherRows : RoutedRows {
+  const T *x;
+  int top_k, K;
+  __device__ uint2 load(int m, int k) const { return *reinterpret_cast<const uint2 *>(x + static_cast<int64_t>(rows[m] / top_k) * K + k); }
+};
+// down: T(T(silu(gate)) * up) of h [T * top_k, 2K] (gate | up), entry e reads row e -- silu_mul2, the MoE decode kernel's
+template <typename T>
+struct SiluMulRows : RoutedRows {
+  const T *h;
+  int K;
+  __device__ uint2 load(int m, int k) const {
+    const T *row = h + static_cast<int64_t>(rows[m]) * (2 * K) + k;
+    const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + K));
+    return make_uint2(silu_mul2<T>(gate.x, up.x), silu_mul2<T>(gate.y, up.y));
+  }
+};
+
+template <typename T, typename Rows>
+__global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__restrict__ out, const uint8_t *__restrict__ raw_base,
+                                                           long long raw_part_bytes, long long out_part_elems, int M_store, int nt, int K,
                                                            int krot, int n_parts) {
   constexpr int G = 128, RB = 8;
   __shared__ __align__(16) uint4 tile[4][G];
@@ -242,16 +288,20 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const T *__restrict__
     return (static_cast<int64_t>(tb) * (K / 16) + (k >> 4)) * (static_cast<int64_t>(nt) * 16) + ((k >> 3) & 1) * (nt * 8) + (n >> 3) * 64 + (n & 7) * 8 +
            (k & 7);
   };
-  if (row0 >= M) {   // a block of padding rows: zeros, in place
+  if (src.skip(row0)) return;
+  if (src.padding_block(row0)) {   // a block of padding rows: zeros, in place
 #pragma unroll
     for (int r = 0; r < RB; ++r) *reinterpret_cast<uint2 *>(o + tiled(row0 + r, g * G + lane * 4)) = make_uint2(0u, 0u);
     return;
   }
   // ---- everything this warp will need from global memory, issued together
   uint2 xr[RB];
+  bool ok[RB];
 #pragma unroll
-  for (int r = 0; r < RB; ++r)
-    xr[r] = row0 + r < M ? *reinterpret_cast<const uint2 *>(x + static_cast<int64_t>(row0 + r) * K + g * G + lane * 4) : make_uint2(0u, 0u);
+  for (int r = 0; r < RB; ++r) {
+    ok[r] = src.valid(row0 + r);
+    xr[r] = ok[r] ? src.load(row0 + r, g * G + lane * 4) : make_uint2(0u, 0u);
+  }
   const uint2 scw = *reinterpret_cast<const uint2 *>(scales + g * G + lane * 4);
   for (int r0 = 0; r0 < krot; r0 += 8) {
     int ij[8][2];
@@ -316,7 +366,7 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const T *__restrict__
   for (int r = 0; r < RB; ++r) {
     const int n = row0 + r, k = g * G + lane * 4;
     uint2 w = make_uint2(0u, 0u);
-    if (n < M) {
+    if (ok[r]) {
       T *pw = reinterpret_cast<T *>(&w);
 #pragma unroll
       for (int c = 0; c < 4; ++c) pw[c] = v[r][c];
@@ -333,17 +383,50 @@ int rotate_small_launch(const void *x, void *out, const void *raw_base, long lon
   const long long blocks = (tasks + 3) / 4;
   if (blocks > 0x7FFFFFFF) { set_error("rotate: too many rows"); return PARO_EINVAL; }
   const long long part_elems = static_cast<long long>(M_store) * K;
+  const uint8_t *raw = static_cast<const uint8_t *>(raw_base);
   if (dtype == PARO_F16)
-    rotate_small_kernel<__half><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(static_cast<const __half *>(x), static_cast<__half *>(out),
-                                                                                  static_cast<const uint8_t *>(raw_base), raw_part_bytes, part_elems,
-                                                                                  static_cast<int>(M), static_cast<int>(M_store), nt, K, krot, n_parts);
+    rotate_small_kernel<__half><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
+        DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), K}, static_cast<__half *>(out), raw, raw_part_bytes, part_elems,
+        static_cast<int>(M_store), nt, K, krot, n_parts);
   else
     rotate_small_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
-        static_cast<const __nv_bfloat16 *>(x), static_cast<__nv_bfloat16 *>(out), static_cast<const uint8_t *>(raw_base), raw_part_bytes, part_elems,
-        static_cast<int>(M), static_cast<int>(M_store), nt, K, krot, n_parts);
+        DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), K}, static_cast<__nv_bfloat16 *>(out), raw,
+        raw_part_bytes, part_elems, static_cast<int>(M_store), nt, K, krot, n_parts);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
   return PARO_OK;
+}
+
+// The pre-pass of a MoE block's grouped GEMM (paro_moe_grouped.cu): the B operand of `rows_max` routing-table positions in tiles
+// of nt, from x [T, K] (silu_mul false: the gate_up operand) or from h [T * top_k, 2K] (silu_mul true: the down operand).
+// raw_base: the rotation every expert shares (expert 0's reference-format region).
+template <typename T>
+static int rotate_routed_T(bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles, int top_k, void *out,
+                           const uint8_t *raw, int rows_max, int nt, int K, int krot, cudaStream_t stream) {
+  const long long blocks = (static_cast<long long>(rows_max / 8) * (K / 128) + 3) / 4;
+  const RoutedRows rr = {rows, live_tiles, nt};
+  T *o = static_cast<T *>(out);
+  if (silu_mul) {
+    SiluMulRows<T> r;
+    static_cast<RoutedRows &>(r) = rr;
+    r.h = static_cast<const T *>(src); r.K = K;
+    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, raw, 0, 0, rows_max, nt, K, krot, 1);
+  } else {
+    GatherRows<T> r;
+    static_cast<RoutedRows &>(r) = rr;
+    r.x = static_cast<const T *>(src); r.top_k = top_k; r.K = K;
+    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, raw, 0, 0, rows_max, nt, K, krot, 1);
+  }
+  PARO_CUDA_OK(cudaGetLastError());
+  note_launches(1);
+  return PARO_OK;
+}
+
+int rotate_routed_launch(bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles, int top_k, void *out, const void *raw_base,
+                         int rows_max, int nt, int K, int krot, int dtype, cudaStream_t stream) {
+  const uint8_t *raw = static_cast<const uint8_t *>(raw_base);
+  if (dtype == PARO_BF16) return rotate_routed_T<__nv_bfloat16>(silu_mul, src, rows, live_tiles, top_k, out, raw, rows_max, nt, K, krot, stream);
+  return rotate_routed_T<__half>(silu_mul, src, rows, live_tiles, top_k, out, raw, rows_max, nt, K, krot, stream);
 }
 
 template <typename T>

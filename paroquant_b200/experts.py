@@ -10,6 +10,7 @@ recomputed per selected expert inside the kernel (it is a prologue of a few micr
 
 `decode_step(T, top_k)` runs the whole block for a decode batch in two launches with the routing read on the device
 (include/paro_b200.h: paro_moe_forward): no host synchronisation, CUDA-graph capturable with the routing changing between replays.
+`prefill_step(T, top_k)` does the same for any T as grouped wgmma GEMMs in six launches (paro_moe_grouped_forward).
 """
 from __future__ import annotations
 
@@ -112,6 +113,10 @@ class ParoExperts:
         """The block for T <= 16 tokens with top_k slots each over fixed device buffers (see ParoMoEStep)."""
         return ParoMoEStep(self, T, top_k)
 
+    def prefill_step(self, T: int, top_k: int) -> "ParoMoEPrefill":
+        """The block for any T >= 1 tokens with top_k slots each over fixed device buffers (see ParoMoEPrefill)."""
+        return ParoMoEPrefill(self, T, top_k)
+
 
 class ParoMoEStep:
     """The expert block of one decode step over fixed device buffers, like ParoChain: write the inputs into `x` [T, hidden],
@@ -124,7 +129,7 @@ class ParoMoEStep:
         dev = experts.packed["gate_up"].device
         self.experts, self.T, self.top_k = experts, int(T), int(top_k)
         self._desc = experts.desc()
-        nbytes = _cabi.moe_workspace_bytes(self._desc, self.T, self.top_k)
+        nbytes = self._workspace_bytes(self._desc, self.T, self.top_k)
         dt = experts.dtype
         self.x = torch.zeros(self.T, experts.hidden, dtype=dt, device=dev)
         self.topk_ids = torch.zeros(self.T, self.top_k, dtype=torch.int32, device=dev)
@@ -135,6 +140,24 @@ class ParoMoEStep:
 
     def step(self) -> torch.Tensor:
         _cabi.moe_forward(self._desc, self.x, self.topk_ids, self.topk_weights, self.h, self.y, self.workspace)
+        return self.y
+
+    __call__ = step
+
+    _workspace_bytes = staticmethod(_cabi.moe_workspace_bytes)
+
+
+class ParoMoEPrefill(ParoMoEStep):
+    """The expert block for any number of tokens (prefill, or decode with more than 16 sequences), with ParoMoEStep's buffers and
+    contract: the routed experts run as grouped INT4 wgmma GEMMs in six launches on the current stream (include/paro_b200.h:
+    paro_moe_grouped_forward), with no host synchronisation and no allocation, so a CUDA graph of `step()` serves every routing.
+    The workspace holds the routing table, the rotated operands and the per-slot expert outputs: about
+    (T * k + n_experts * 128) * max(hidden, I) * 2 + T * k * hidden * 2 bytes at most."""
+
+    _workspace_bytes = staticmethod(_cabi.moe_grouped_workspace_bytes)
+
+    def step(self) -> torch.Tensor:
+        _cabi.moe_grouped_forward(self._desc, self.x, self.topk_ids, self.topk_weights, self.h, self.y, self.workspace)
         return self.y
 
     __call__ = step
