@@ -7,8 +7,7 @@
 #include <cstdlib>
 
 #include "paro_common.cuh"
-#include "paro_layout.h"
-#include "paro_stream.h"
+#include "paro_launch.h"
 
 namespace paro {
 
@@ -22,45 +21,6 @@ void set_error(const char *fmt, ...) {
   va_end(ap);
 }
 void note_launches(int n) { g_launches += n; }
-
-// implemented in the kernel translation units
-int rotate_launch(const void *x, void *out, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
-                  int scales_dtype, int64_t M, int K, int krot, int G, int dtype, cudaStream_t stream);
-int rotate_backward_launch(const void *y, const void *gout, const void *x, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
-                           int scales_dtype, void *grad_x, float *grad_theta, float *grad_scale, int64_t M, int K, int krot, int G, int dtype,
-                           int ref_formula, cudaStream_t stream);
-int prepack_launch(const paro_linear_shape &s, const Layout &L, const int32_t *qweight, const int32_t *qzeros,
-                   const void *scales, int scales_dtype, const int16_t *pairs, const void *theta, int theta_dtype,
-                   const void *cscales, int cs_dtype, void *packed, cudaStream_t stream);
-int unpack_dense_launch(const paro_linear_shape &s, const Layout &L, const void *packed, void *W, cudaStream_t stream);
-bool decode_supported(const Layout &L, int64_t M);
-int decode_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
-                   const void *bias, void *y, void *scratch, size_t scratch_bytes, cudaStream_t stream);
-size_t decode_scratch_bytes(const Layout &L, int64_t max_m);
-int decode_trace_read(unsigned long long *host, int max_ctas);
-int decode_debug_plan(const Layout &L, int64_t M, int sets, int sms, const int32_t *resident4, int32_t *out20);
-bool stream_supported(const Layout &L, int64_t M);
-size_t stream_sync_bytes(const Layout &L);
-size_t stream_workspace_bytes(const Layout &L, int64_t max_m);
-size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M);
-int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream);
-int stream_linear_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M, const void *bias, void *y,
-                          void *workspace, size_t workspace_bytes, cudaStream_t stream);
-int stream_trace_read(unsigned long long *host, int max_ctas);
-int stream_debug_plan(const Layout &L, int64_t M, int sets, int ctas, int32_t *out);
-size_t gemm_workspace_bytes(const Layout &L, int64_t max_m);
-int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out);
-int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
-                 const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream);
-size_t moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);
-int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const float *wts, int64_t T, int32_t k, void *h, void *y,
-                void *workspace, size_t workspace_bytes, cudaStream_t stream);
-int moe_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t sms, int32_t *out);
-int moe_debug_silu_mul(int dtype, const void *gate_up, void *act, int64_t M, int I, cudaStream_t stream);
-size_t moe_grouped_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);
-int moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const float *wts, int64_t T, int32_t k, void *h, void *y,
-                        void *workspace, size_t workspace_bytes, cudaStream_t stream);
-int moe_grouped_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t *out);
 
 const Knobs &knobs() {
   static const Knobs k = [] {

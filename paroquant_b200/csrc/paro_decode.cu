@@ -28,6 +28,7 @@
 #include <mutex>
 #include <type_traits>
 
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"
 
 namespace paro {
@@ -539,9 +540,6 @@ size_t decode_scratch_bytes(const Layout &L, int64_t max_m) {
   return any ? static_cast<size_t>(L.n_parts) * kDecN * L.K * 2 : 0;
 }
 
-int rotate_small_launch(const void *x, void *out, const void *raw_base, long long raw_part_bytes, int n_parts, int64_t M, int64_t M_store, int nt,
-                        int K, int krot, int dtype, cudaStream_t stream);
-
 int decode_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
                    const void *bias, void *y, void *scratch, size_t scratch_bytes, cudaStream_t stream) {
   const int sms = device_sms();
@@ -553,8 +551,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   const size_t part_bytes = static_cast<size_t>(kDecN) * L.K * 2;   // 16 rows (zero padded) x K of T, B-operand order
   const bool prerot = decode_wants_prerot(L, M) && scratch && scratch_bytes >= L.n_parts * part_bytes;
   if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_small_kernel)
-    const int rc = rotate_small_launch(x, scratch, static_cast<const uint8_t *>(packed) + L.raw_off, static_cast<long long>(L.raw_part_bytes), L.n_parts, M,
-                                       kDecN, kDecN, L.K, L.krot, s.dtype, stream);
+    const int rc = rotate_small_launch(L, packed, x, scratch, M, kDecN, kDecN, stream);
     if (rc) return rc;
   }
   DecParams p = {};

@@ -18,12 +18,10 @@
 // The same kernel serves the MoE block's grouped GEMMs (paro_moe_grouped.cu) through its tile source: there a token block is a
 // tile slot of the routing table -- NT sorted (token, slot) rows of one expert -- the weights are that expert's, and the
 // epilogue scatters each row to its (token, slot) output row.
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"
 
 namespace paro {
-
-int rotate_small_launch(const void *x, void *out, const void *raw_base, long long raw_part_bytes, int n_parts, int64_t M, int64_t M_store, int nt,
-                        int K, int krot, int dtype, cudaStream_t stream);
 
 constexpr int kGemmConsumers = 2;                         // warpgroups of 64 output columns
 constexpr int kGemmThreads = 128 * (1 + kGemmConsumers);
@@ -302,8 +300,7 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
   // ---- pre-pass: ONE launch rotates x for every partition, output in B-operand tile order (paro_rotate.cu: rotate_small_kernel
   // fetches all stage parameters up front; the per-partition rotate_kernel launches it replaces cost 3 x ~7 us at 256 tokens)
   {
-    const int rc = rotate_small_launch(x, xr_base, pk + L.raw_off, static_cast<long long>(L.raw_part_bytes), L.n_parts, M, m_pad, NT, L.K, L.krot, s.dtype,
-                                       stream);
+    const int rc = rotate_small_launch(L, pk, x, xr_base, M, m_pad, NT, stream);
     if (rc) return rc;
   }
   GemmParams p;

@@ -1,12 +1,13 @@
 // The streaming layout paro_prepack writes and both fused kernels read.  Host + device.
 //
-//   packed := [ rotation metadata ][ weight records ][ rotation metadata, reference format ]
+//   packed := [ rotation metadata ][ weight records ]
 //
-// Rotation metadata, one block per (partition p, group gk), groups of 128 channels:
-//   [r = 0..krot-1][128] uint8   pair indices: (i, j) of pair t at bytes 2t, 2t+1
+// Rotation metadata, one block per (partition p, group gk), groups of 128 channels (offsets: meta_pairs_off & co. below):
+//   [r = 0..krot-1][128] uint8   pair indices: (i, j) of pair t at bytes 2t, 2t+1, always inside the 128-channel group
 //   [r = 0..krot-1][ 64] T       theta, already cast to the activation dtype T (rotation.cu:75)
 //   [128]                T       channel scales, cast to T (rotation.cu:76-78)
-//   -> krot*256 + 256 bytes; lane l of the warp that owns the group reads 4 bytes of each row.
+//   -> krot*256 + 256 bytes; lane l of the warp that owns the group reads 4 bytes of each stage's pair and theta rows
+//   (pairs 2l and 2l + 1) and 8 bytes of the scales (channels 4l .. 4l + 3).  Every rotation path reads these blocks.
 //
 // Weight records.  N is cut into BLOCKS of 128 output columns per partition (a last partial block is
 // zero-filled), K into the quantisation groups of 128 channels.  One record = one (block, group gk) =
@@ -57,6 +58,11 @@ PARO_HD constexpr int block_zero_off(int qhalves) { return kBlockScaleOff + qhal
 PARO_HD constexpr int frag_offset(int tile, int kh, int lane) { return ((tile * 2 + kh) * 32 + lane) * 16; }
 // entry of block column `col` (0..127) in a scale / zero set: rows g and g + 8 of a 16-row tile side by side
 PARO_HD constexpr int qparam_index(int col) { return (col & ~15) | ((col & 7) << 1) | ((col >> 3) & 1); }
+// byte offsets inside one group's rotation metadata block: stage r's pair indices ([128] uint8) and theta ([64] T), the channel
+// scales ([128] T)
+PARO_HD constexpr int meta_pairs_off(int r) { return r * 128; }
+PARO_HD constexpr int meta_theta_off(int krot, int r) { return krot * 128 + r * 128; }
+PARO_HD constexpr int meta_scales_off(int krot) { return krot * 256; }
 
 struct Layout {
   int K, N, krot, n_parts, dtype;
@@ -66,7 +72,7 @@ struct Layout {
   int part_col_begin[PARO_MAX_PARTS + 1];   // first output column of each partition
   int part_block_begin[PARO_MAX_PARTS + 1]; // cumulative blocks per partition
   int meta_group_bytes;                     // krot*256 + 256
-  size_t meta_off, rec_off, raw_off, raw_part_bytes, total_bytes;  // raw_*: rotation metadata again, in torch.ops.rotation.rotate's own format
+  size_t meta_off, rec_off, total_bytes;
 
   PARO_HD size_t meta_offset(int part, int gk) const {
     return meta_off + (static_cast<size_t>(part) * groups + gk) * meta_group_bytes;
@@ -113,14 +119,11 @@ inline bool make_layout(const paro_linear_shape &s, Layout &L, const char **why)
   }
   if (n != s.out_features) { *why = msgs[4]; return false; }
   L.blocks_total = nb;
-  L.meta_group_bytes = s.krot * 256 + 256;
+  L.meta_group_bytes = meta_scales_off(s.krot) + 256;
   L.meta_off = 0;
   size_t meta = static_cast<size_t>(s.n_parts) * L.groups * L.meta_group_bytes;
   L.rec_off = (meta + 127) / 128 * 128;
-  L.raw_off = (L.rec_off + static_cast<size_t>(L.blocks_total) * L.groups * L.rec_bytes + 127) / 128 * 128;
-  // per partition: pairs int16 [krot][K], theta T [krot][K/2], channel scales T [K] (the large-M pre-pass reads these)
-  L.raw_part_bytes = (static_cast<size_t>(s.krot) * L.K * 3 + static_cast<size_t>(L.K) * 2 + 127) / 128 * 128;
-  L.total_bytes = L.raw_off + L.raw_part_bytes * s.n_parts;
+  L.total_bytes = L.rec_off + static_cast<size_t>(L.blocks_total) * L.groups * L.rec_bytes;
   return true;
 }
 

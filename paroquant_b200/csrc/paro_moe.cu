@@ -28,6 +28,7 @@
 #include <cstring>
 #include <type_traits>
 
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"
 
 namespace paro {

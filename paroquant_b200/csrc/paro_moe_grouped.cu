@@ -21,14 +21,10 @@
 //
 // The grids are sized for the worst routing: at most floor(T k / NT) + min(E, T k) tiles are live.  NT is chosen on the host
 // from (T, k, E) only, so one plan serves every routing and a captured CUDA graph stays valid while the ids change.
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"
 
 namespace paro {
-
-int rotate_routed_launch(bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles, int top_k, void *out, const void *raw_base,
-                         int rows_max, int nt, int K, int krot, int dtype, cudaStream_t stream);
-int gemm_grouped_launch(const Layout &L, const void *packed, long long expert_stride, const void *xr, void *y, int NT, int slots,
-                        const int32_t *rows, const int32_t *tile_expert, const int32_t *live_tiles, int dtype, cudaStream_t stream);
 
 constexpr int kGroupedMaxEntries = PARO_MOE_GROUPED_MAX_ENTRIES;   // T * top_k
 constexpr int kGroupedMaxExperts = PARO_MOE_GROUPED_MAX_EXPERTS;   // one route thread per expert
@@ -248,11 +244,11 @@ int moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *id
   moe_route_kernel<<<1, kRouteThreads, kRouteWarps * ms.E * 4, stream>>>(ids, n, ms.E, gp.nt, rows, tile_expert, live);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
-  if ((rc = rotate_routed_launch(false, x, rows, live, k, operand, gu + ms.gu.raw_off, rows_max, gp.nt, ms.H, ms.gu.krot, dtype, stream))) return rc;
+  if ((rc = rotate_routed_launch(ms.gu, gu, false, x, rows, live, k, operand, rows_max, gp.nt, stream))) return rc;
   if ((rc = gemm_grouped_launch(ms.gu, gu, static_cast<long long>(d->gate_up_stride), operand, h, gp.nt, gp.slots, rows, tile_expert, live, dtype,
                                 stream)))
     return rc;
-  if ((rc = rotate_routed_launch(true, h, rows, live, k, operand, dn + ms.dn.raw_off, rows_max, gp.nt, ms.I, ms.dn.krot, dtype, stream))) return rc;
+  if ((rc = rotate_routed_launch(ms.dn, dn, true, h, rows, live, k, operand, rows_max, gp.nt, stream))) return rc;
   if ((rc = gemm_grouped_launch(ms.dn, dn, static_cast<long long>(d->down_stride), operand, ys, gp.nt, gp.slots, rows, tile_expert, live, dtype,
                                 stream)))
     return rc;

@@ -3,7 +3,7 @@
 // reaches through ParoQuantLinearMethod.process_weights_after_loading
 // (/root/reference/paroquant/inference/backends/vllm/plugin.py:208-279).
 #include "paro_common.cuh"
-#include "paro_layout.h"
+#include "paro_launch.h"
 
 namespace paro {
 
@@ -41,27 +41,14 @@ __global__ void prepack_meta_kernel(Layout L, const int16_t *__restrict__ pairs,
   const int16_t lift = (L.qhalves == 2 && c >= 64) ? 64 : 0, imask = L.qhalves == 2 ? 0x3F : 0x7F;
   for (int r = 0; r < L.krot; ++r) {
     const int16_t v = static_cast<int16_t>((pairs[(static_cast<int64_t>(part) * L.krot + r) * K + gk * kGroup + c] & imask) + lift);
-    blk[r * 128 + c] = static_cast<uint8_t>(v);
+    blk[meta_pairs_off(r) + c] = static_cast<uint8_t>(v);
     if (c < 64) {
       const int64_t ti = (static_cast<int64_t>(part) * L.krot + r) * (K / 2) + gk * 64 + c;
-      reinterpret_cast<uint16_t *>(blk + L.krot * 128)[r * 64 + c] = cast_to_T_bits(theta, ti, theta_dtype, L.dtype);
+      reinterpret_cast<uint16_t *>(blk + meta_theta_off(L.krot, r))[c] = cast_to_T_bits(theta, ti, theta_dtype, L.dtype);
     }
   }
-  const uint16_t csb = cast_to_T_bits(cscales, static_cast<int64_t>(part) * K + gk * kGroup + c, cs_dtype, L.dtype);
-  reinterpret_cast<uint16_t *>(blk + L.krot * 256)[c] = csb;
-  // second copy in the reference op's own format (int16 pairs, [krot][K/2] theta, [K] scales), theta / scales in T
-  uint8_t *raw = packed + L.raw_off + part * L.raw_part_bytes;
-  int16_t *rp = reinterpret_cast<int16_t *>(raw);
-  uint16_t *rt = reinterpret_cast<uint16_t *>(raw + static_cast<size_t>(L.krot) * K * 2);
-  uint16_t *rs = reinterpret_cast<uint16_t *>(raw + static_cast<size_t>(L.krot) * K * 3);
-  for (int r = 0; r < L.krot; ++r) {
-    rp[static_cast<int64_t>(r) * K + gk * kGroup + c] =
-        static_cast<int16_t>(pairs[(static_cast<int64_t>(part) * L.krot + r) * K + gk * kGroup + c] + lift);   // the pre-pass always runs with groups of 128
-    if (c < 64)
-      rt[static_cast<int64_t>(r) * (K / 2) + gk * 64 + c] =
-          cast_to_T_bits(theta, (static_cast<int64_t>(part) * L.krot + r) * (K / 2) + gk * 64 + c, theta_dtype, L.dtype);
-  }
-  rs[gk * kGroup + c] = csb;
+  reinterpret_cast<uint16_t *>(blk + meta_scales_off(L.krot))[c] =
+      cast_to_T_bits(cscales, static_cast<int64_t>(part) * K + gk * kGroup + c, cs_dtype, L.dtype);
 }
 
 // block index over all partitions -> partition

@@ -12,6 +12,7 @@
 // loads and two 128-bit stores for all RB rows at once.  The 16-byte slot of channel c is
 // c ^ ((c >> 3) & 7), which makes the coalesced transpose-in / transpose-out conflict free.
 #include "paro_common.cuh"
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"   // silu_mul2: the MoE down pre-pass
 
 namespace paro {
@@ -61,7 +62,7 @@ template <typename T, int G>
 __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T *__restrict__ out,
                                                      const int16_t *__restrict__ idx, const void *__restrict__ theta,
                                                      int theta_dtype, const void *__restrict__ scales, int scales_dtype,
-                                                     int64_t M, int K, int krot, int64_t M_store, int tiled_nt) {
+                                                     int64_t M, int K, int krot) {
   constexpr int RB = RotVec<T>::RB;
   constexpr int CPL = G / 32;  // channels per lane for the coalesced load / store
   constexpr int PPL = G / 64;  // pairs per lane
@@ -70,7 +71,7 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int groups = K / G;
   const int64_t task = static_cast<int64_t>(blockIdx.x) * 4 + warp;
-  const int64_t row_blocks = (M_store + RB - 1) / RB;  // rows in [M, M_store) are zero padding (tiled output only)
+  const int64_t row_blocks = (M + RB - 1) / RB;
   if (task >= row_blocks * groups) return;
   const int g = static_cast<int>(task % groups);
   const int64_t row0 = (task / groups) * RB;
@@ -184,23 +185,13 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
     }
 #pragma unroll
     for (int r = 0; r < RB; ++r)
-      if (row0 + r < M_store) {
+      if (row0 + r < M) {
         if constexpr (CPL == 4) {
           uint2 raw;
           T *pr = reinterpret_cast<T *>(&raw);
 #pragma unroll
           for (int c = 0; c < 4; ++c) pr[c] = v[r][c];
-          if (tiled_nt) {
-            // B-operand order of the wgmma GEMM (paro_gemm.cu): [token block][k16 step][k half][n/8][n%8][8 elems]
-            const int64_t m = row0 + r;
-            const int64_t tb = m / tiled_nt;
-            const int n = static_cast<int>(m - tb * tiled_nt), k = g * G + lane * 4;
-            const int64_t off = (tb * (K / 16) + (k >> 4)) * (static_cast<int64_t>(tiled_nt) * 16) + ((k >> 3) & 1) * (tiled_nt * 8) +
-                                (n >> 3) * 64 + (n & 7) * 8 + (k & 7);
-            *reinterpret_cast<uint2 *>(out + off) = raw;
-          } else {
-            *reinterpret_cast<uint2 *>(out + (row0 + r) * K + g * G + lane * 4) = raw;
-          }
+          *reinterpret_cast<uint2 *>(out + (row0 + r) * K + g * G + lane * 4) = raw;
         } else {
           uint32_t raw;
           T *pr = reinterpret_cast<T *>(&raw);
@@ -217,7 +208,8 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
 // ONE launch for all partitions of a merged linear: warp = (partition, group, block of 8 rows); output in the B-operand order
 // of the consumer (tiles of nt tokens, padding rows zero).  Same arithmetic as rotate_kernel; what differs is latency: the pair
 // indices and angles of all (<= 8 at a time) rotations are fetched up front, so the launch costs one global-load round trip
-// instead of one per stage (rotate_kernel at 16 rows: ~7 us, almost all of it eight dependent L2 / DRAM latencies).
+// instead of one per stage (rotate_kernel at 16 rows: ~7 us, almost all of it eight dependent L2 / DRAM latencies).  The
+// metadata is the packed layout's per-group blocks (paro_layout.h), read with the loads fetch_meta makes in the fused kernels.
 //
 // A row source says what feeds output row m: `skip(row0)` -- the block of 8 rows from row0 on is never read, leave it;
 // `padding_block(row0)` -- all 8 rows are padding, store zeros; `valid(m)` -- row m has an input (else it is a zero row);
@@ -264,8 +256,8 @@ struct SiluMulRows : RoutedRows {
 };
 
 template <typename T, typename Rows>
-__global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__restrict__ out, const uint8_t *__restrict__ raw_base,
-                                                           long long raw_part_bytes, long long out_part_elems, int M_store, int nt, int K,
+__global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__restrict__ out, const uint8_t *__restrict__ meta,
+                                                           int meta_group_bytes, long long out_part_elems, int M_store, int nt, int K,
                                                            int krot, int n_parts) {
   constexpr int G = 128, RB = 8;
   __shared__ __align__(16) uint4 tile[4][G];
@@ -275,10 +267,7 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
   const long long task = static_cast<long long>(blockIdx.x) * 4 + warp;          // (part, row block, group)
   if (task >= static_cast<long long>(n_parts) * row_blocks * groups) return;
   const int g = static_cast<int>(task % groups), rb = static_cast<int>((task / groups) % row_blocks), part = static_cast<int>(task / (static_cast<long long>(row_blocks) * groups));
-  const uint8_t *raw = raw_base + part * raw_part_bytes;
-  const int16_t *idx = reinterpret_cast<const int16_t *>(raw);
-  const T *theta = reinterpret_cast<const T *>(raw + static_cast<size_t>(krot) * K * 2);
-  const T *scales = reinterpret_cast<const T *>(raw + static_cast<size_t>(krot) * K * 3);
+  const uint8_t *blk = meta + (static_cast<long long>(part) * groups + g) * meta_group_bytes;   // this (partition, group)'s block
   T *o = out + part * out_part_elems;
   uint4 *rot = tile[warp];
   const int row0 = rb * RB;
@@ -302,17 +291,14 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
     ok[r] = src.valid(row0 + r);
     xr[r] = ok[r] ? src.load(row0 + r, g * G + lane * 4) : make_uint2(0u, 0u);
   }
-  const uint2 scw = *reinterpret_cast<const uint2 *>(scales + g * G + lane * 4);
+  const uint2 scw = *reinterpret_cast<const uint2 *>(blk + meta_scales_off(krot) + 8 * lane);
   for (int r0 = 0; r0 < krot; r0 += 8) {
-    int ij[8][2];
-    uint32_t th[8];
+    uint32_t iw[8], th[8];   // stage r0 + r: bytes (i0, j0, i1, j1) of pairs 2 lane, 2 lane + 1, and their two angles
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
       if (r0 + r < krot) {
-        const uint2 w = *reinterpret_cast<const uint2 *>(idx + static_cast<int64_t>(r0 + r) * K + g * G + 4 * lane);   // pairs 2 lane, 2 lane + 1
-        ij[r][0] = static_cast<int>(w.x);
-        ij[r][1] = static_cast<int>(w.y);
-        th[r] = *reinterpret_cast<const uint32_t *>(theta + static_cast<int64_t>(r0 + r) * (K / 2) + g * (G / 2) + 2 * lane);
+        iw[r] = *reinterpret_cast<const uint32_t *>(blk + meta_pairs_off(r0 + r) + 4 * lane);
+        th[r] = *reinterpret_cast<const uint32_t *>(blk + meta_theta_off(krot, r0 + r) + 4 * lane);
       }
     }
     if (r0 == 0) {
@@ -343,7 +329,7 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
         for (int q = 0; q < 2; ++q) {
           float sn, cs;
           __sincosf(q ? t2.y : t2.x, &sn, &cs);
-          const int pi = ij[r][q] & 0xFFFF, pj = (ij[r][q] >> 16) & 0xFFFF;
+          const int pi = (iw[r] >> (16 * q)) & 0xFF, pj = (iw[r] >> (16 * q + 8)) & 0xFF;
           uint4 vi = rot[rot_slot(pi)], vj = rot[rot_slot(pj)];
           pair_update<T>(vi, vj, cs, sn);
           rot[rot_slot(pi)] = vi;
@@ -375,23 +361,23 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
   }
 }
 
-// all partitions in one launch; metadata in the layout's reference-format region (theta and channel scales already of dtype T);
-// output per partition: M_store rows (a multiple of 8; rows >= M zero) in tiles of `nt` tokens
-int rotate_small_launch(const void *x, void *out, const void *raw_base, long long raw_part_bytes, int n_parts, int64_t M, int64_t M_store, int nt,
-                        int K, int krot, int dtype, cudaStream_t stream) {
-  const long long tasks = static_cast<long long>(n_parts) * (M_store / 8) * (K / 128);
+// all partitions of L in one launch, x [M, K] -> out: per partition M_store rows (a multiple of 8; rows >= M zero) in tiles of
+// `nt` tokens
+int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
+  const int K = L.K;
+  const long long tasks = static_cast<long long>(L.n_parts) * (M_store / 8) * (K / 128);
   const long long blocks = (tasks + 3) / 4;
   if (blocks > 0x7FFFFFFF) { set_error("rotate: too many rows"); return PARO_EINVAL; }
   const long long part_elems = static_cast<long long>(M_store) * K;
-  const uint8_t *raw = static_cast<const uint8_t *>(raw_base);
-  if (dtype == PARO_F16)
+  const uint8_t *meta = static_cast<const uint8_t *>(packed) + L.meta_off;
+  if (L.dtype == PARO_F16)
     rotate_small_kernel<__half><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
-        DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), K}, static_cast<__half *>(out), raw, raw_part_bytes, part_elems,
-        static_cast<int>(M_store), nt, K, krot, n_parts);
+        DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), K}, static_cast<__half *>(out), meta, L.meta_group_bytes,
+        part_elems, static_cast<int>(M_store), nt, K, L.krot, L.n_parts);
   else
     rotate_small_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
-        DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), K}, static_cast<__nv_bfloat16 *>(out), raw,
-        raw_part_bytes, part_elems, static_cast<int>(M_store), nt, K, krot, n_parts);
+        DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), K}, static_cast<__nv_bfloat16 *>(out), meta,
+        L.meta_group_bytes, part_elems, static_cast<int>(M_store), nt, K, L.krot, L.n_parts);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
   return PARO_OK;
@@ -399,10 +385,11 @@ int rotate_small_launch(const void *x, void *out, const void *raw_base, long lon
 
 // The pre-pass of a MoE block's grouped GEMM (paro_moe_grouped.cu): the B operand of `rows_max` routing-table positions in tiles
 // of nt, from x [T, K] (silu_mul false: the gate_up operand) or from h [T * top_k, 2K] (silu_mul true: the down operand).
-// raw_base: the rotation every expert shares (expert 0's reference-format region).
+// The rotation every expert shares is partition 0's of expert 0 (`packed`); gate and up share it.
 template <typename T>
-static int rotate_routed_T(bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles, int top_k, void *out,
-                           const uint8_t *raw, int rows_max, int nt, int K, int krot, cudaStream_t stream) {
+static int rotate_routed_T(const Layout &L, const uint8_t *meta, bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles,
+                           int top_k, void *out, int rows_max, int nt, cudaStream_t stream) {
+  const int K = L.K;
   const long long blocks = (static_cast<long long>(rows_max / 8) * (K / 128) + 3) / 4;
   const RoutedRows rr = {rows, live_tiles, nt};
   T *o = static_cast<T *>(out);
@@ -410,32 +397,30 @@ static int rotate_routed_T(bool silu_mul, const void *src, const int32_t *rows, 
     SiluMulRows<T> r;
     static_cast<RoutedRows &>(r) = rr;
     r.h = static_cast<const T *>(src); r.K = K;
-    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, raw, 0, 0, rows_max, nt, K, krot, 1);
+    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, meta, L.meta_group_bytes, 0, rows_max, nt, K, L.krot, 1);
   } else {
     GatherRows<T> r;
     static_cast<RoutedRows &>(r) = rr;
     r.x = static_cast<const T *>(src); r.top_k = top_k; r.K = K;
-    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, raw, 0, 0, rows_max, nt, K, krot, 1);
+    rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(r, o, meta, L.meta_group_bytes, 0, rows_max, nt, K, L.krot, 1);
   }
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
   return PARO_OK;
 }
 
-int rotate_routed_launch(bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles, int top_k, void *out, const void *raw_base,
-                         int rows_max, int nt, int K, int krot, int dtype, cudaStream_t stream) {
-  const uint8_t *raw = static_cast<const uint8_t *>(raw_base);
-  if (dtype == PARO_BF16) return rotate_routed_T<__nv_bfloat16>(silu_mul, src, rows, live_tiles, top_k, out, raw, rows_max, nt, K, krot, stream);
-  return rotate_routed_T<__half>(silu_mul, src, rows, live_tiles, top_k, out, raw, rows_max, nt, K, krot, stream);
+int rotate_routed_launch(const Layout &L, const void *packed, bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles,
+                         int top_k, void *out, int rows_max, int nt, cudaStream_t stream) {
+  const uint8_t *meta = static_cast<const uint8_t *>(packed) + L.meta_off;
+  if (L.dtype == PARO_BF16) return rotate_routed_T<__nv_bfloat16>(L, meta, silu_mul, src, rows, live_tiles, top_k, out, rows_max, nt, stream);
+  return rotate_routed_T<__half>(L, meta, silu_mul, src, rows, live_tiles, top_k, out, rows_max, nt, stream);
 }
 
 template <typename T>
 static int launch_T(const void *x, void *out, const int16_t *idx, const void *theta, int theta_dtype,
-                    const void *scales, int scales_dtype, int64_t M, int K, int krot, int G, cudaStream_t stream,
-                    int64_t M_store = -1, int tiled_nt = 0) {
+                    const void *scales, int scales_dtype, int64_t M, int K, int krot, int G, cudaStream_t stream) {
   constexpr int RB = RotVec<T>::RB;
-  if (M_store < 0) M_store = M;
-  const int64_t tasks = ((M_store + RB - 1) / RB) * (K / G);
+  const int64_t tasks = ((M + RB - 1) / RB) * (K / G);
   const int64_t blocks = (tasks + 3) / 4;
   if (blocks > 0x7FFFFFFF) {
     set_error("rotate: too many rows");
@@ -445,10 +430,10 @@ static int launch_T(const void *x, void *out, const int16_t *idx, const void *th
   T *op = static_cast<T *>(out);
   if (G == 128)
     rotate_kernel<T, 128><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(xp, op, idx, theta, theta_dtype, scales,
-                                                                            scales_dtype, M, K, krot, M_store, tiled_nt);
+                                                                            scales_dtype, M, K, krot);
   else
     rotate_kernel<T, 64><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(xp, op, idx, theta, theta_dtype, scales,
-                                                                           scales_dtype, M, K, krot, M_store, tiled_nt);
+                                                                           scales_dtype, M, K, krot);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
   return PARO_OK;
@@ -649,15 +634,6 @@ int rotate_backward_launch(const void *y, const void *gout, const void *x, const
   }
   set_error("rotate supports Float, Half, and BFloat16, got dtype code %d", dtype);
   return PARO_EINVAL;
-}
-
-// Rotation pre-pass of the large-M path: the raw metadata of ONE partition, output in the B-operand tile
-// order of the wgmma GEMM, zero rows up to M_store (a multiple of tiled_nt).
-int rotate_tiled_launch(const void *x, void *out, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
-                        int scales_dtype, int64_t M, int64_t M_store, int tiled_nt, int K, int krot, int dtype, cudaStream_t stream) {
-  if (dtype == PARO_F16)
-    return launch_T<__half>(x, out, idx, theta, theta_dtype, scales, scales_dtype, M, K, krot, 128, stream, M_store, tiled_nt);
-  return launch_T<__nv_bfloat16>(x, out, idx, theta, theta_dtype, scales, scales_dtype, M, K, krot, 128, stream, M_store, tiled_nt);
 }
 
 }  // namespace paro

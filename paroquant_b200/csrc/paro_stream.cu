@@ -39,8 +39,8 @@
 #include <type_traits>
 #include <vector>
 
+#include "paro_launch.h"
 #include "paro_tc_common.cuh"
-#include "paro_stream.h"
 
 namespace paro {
 

@@ -328,6 +328,8 @@ __device__ __forceinline__ void sincos2(uint32_t theta_pair_bits, float &c0, flo
 // ------------------------------------------------------------------ rotation prologue of the small-M kernels
 // One group's rotation metadata (paro_layout.h) as this lane uses it: its 4 channel scales and, for krot = 8, its pair-index
 // and theta words of every stage -- fetched with the scales, so they fly during whatever the kernel waits for before x.
+// Here and in rotation_tasks the block offsets meta_pairs_off(r), meta_theta_off(krot, r) and meta_scales_off(krot) are written
+// out: through the helpers nvcc orders the address arithmetic differently and the fused kernels' SASS changes.
 struct RotMeta {
   uint32_t idxw[8], tw[8];
   uint2 csw;

@@ -55,17 +55,16 @@ def test_struct_layout_matches_header():
 def test_size_queries_and_shape_errors():
     s = _cabi.make_shape(4096, [4096], 128, 8, torch.bfloat16)
     # 32 blocks of 128 columns x 32 groups x 8576-byte records + 32 groups x (8*256+256) bytes of rotation metadata
-    raw = lambda K, P: P * ((8 * K * 3 + 2 * K + 127) // 128 * 128)      # reference-format rotation metadata (GEMM pre-pass)
-    assert _cabi.packed_bytes(s) == 32 * 32 * 8576 + 32 * 2304 + raw(4096, 1)
+    assert _cabi.packed_bytes(s) == 32 * 32 * 8576 + 32 * 2304
     assert _cabi.workspace_bytes(s, 1) >= 256          # the small-M kernel reduces through distributed shared memory
     assert _cabi.workspace_bytes(s, 4096) >= 4096 * 4096 * 2   # M > 16: the rotated activations are staged once
     assert _cabi.workspace_bytes(s, 16) >= _cabi.workspace_bytes(s, 8)
     # a partition that is not a whole number of 128-column blocks is padded to one
     s2 = _cabi.make_shape(256, [272, 16], 128, 8, torch.float16)
-    assert _cabi.packed_bytes(s2) == (3 + 1) * 2 * 8576 + 2 * 2 * 2304 + raw(256, 2)
+    assert _cabi.packed_bytes(s2) == (3 + 1) * 2 * 8576 + 2 * 2 * 2304
     # group_size 64: a record still covers 128 channels and carries two scale / zero sets (8960 bytes)
     s64 = _cabi.make_shape(4096, [4096], 64, 8, torch.bfloat16)
-    assert _cabi.packed_bytes(s64) == 32 * 32 * 8960 + 32 * 2304 + raw(4096, 1)
+    assert _cabi.packed_bytes(s64) == 32 * 32 * 8960 + 32 * 2304
     for bad, msg in ((dict(in_features=4000), "multiple of 128"), (dict(part_sizes=[100]), "multiple of 16"),
                      (dict(group_size=32), "group_size"), (dict(krot=17), "krot")):
         kw = dict(in_features=4096, part_sizes=[4096], group_size=128, krot=8, dtype=torch.bfloat16)
@@ -78,7 +77,7 @@ def test_size_queries_and_shape_errors():
 
 def test_merged_layout_is_partition_major():
     s = _cabi.make_shape(4096, [4096, 1024, 1024], 128, 8, torch.float16)
-    assert _cabi.packed_bytes(s) == 32 * 48 * 8576 + ((3 * 32 * 2304 + 127) // 128) * 128 + 3 * ((8 * 4096 * 3 + 2 * 4096 + 127) // 128 * 128)
+    assert _cabi.packed_bytes(s) == 32 * 48 * 8576 + ((3 * 32 * 2304 + 127) // 128) * 128
 
 
 def test_cpu_tensors_are_rejected_loudly():

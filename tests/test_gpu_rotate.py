@@ -233,3 +233,44 @@ def test_fused_backward_vs_oracle_both_theta_formulas(ops, oracle, G):
     a = _cabi.rotate_backward(y, go, x, pr, th, sc, G)[1]
     b = _cabi.rotate_backward(y, go, x, pr, th, sc, G, reference_formula=True)[1]
     assert (a - b).norm() / a.norm() > 1e-2          # the two really differ on random data
+
+
+# (K, partitions, M, group, krot, dtype): the decode pre-pass (M <= 16: 16 rows in tiles of 16) and the GEMM's (M > 16: m_pad rows in
+# tiles of the GEMM's NT); krot 9 and 16 run a second chunk of 8 stages
+PREPASS_CASES = [
+    (1024, [512], 5, 128, 9, torch.bfloat16),
+    (2048, [256, 128, 384], 16, 64, 16, torch.float16),
+    (1024, [384], 48, 64, 3, torch.bfloat16),
+    (1536, [1024, 256, 256], 300, 128, 16, torch.float16),
+    (512, [256], 300, 64, 9, torch.bfloat16),
+]
+
+
+@pytest.mark.parametrize("K,parts,M,G,krot,dt", PREPASS_CASES)
+def test_prepass_operand_is_the_rotate_op_bit_for_bit(ops, K, parts, M, G, krot, dt):
+    """The tensor-core kernels' pre-pass (rotate_small_kernel, reading the packed layout's metadata blocks) writes, for every
+    partition, exactly torch.ops.rotation.rotate of the same rows in the B-operand tile order, padding rows zero."""
+    import ctypes
+    from paroquant_b200 import _cabi
+    from paroquant_b200.linear import ParoLinearKernel
+    L = make_synthetic_layer(K, parts, group_size=G, krot=krot, seed=600 + M, device="cuda")
+    k = ParoLinearKernel.from_buffers(L, dt, max_m=M, private_workspace=True)
+    x = make_synthetic_activations(M, K, seed=610 + M, device="cuda", dtype=dt)
+    k(x)
+    assert _cabi.last_launch_count() == 2   # pre-pass + consumer: the rows below were rotated by the pre-pass
+    if M <= 16:
+        nt = rows = 16
+    else:
+        plan = (ctypes.c_int32 * 2)()
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        assert _cabi.lib().paro_debug_gemm_plan(ctypes.byref(k.shape), M, sms, plan) == 0
+        nt = plan[0]
+        rows = (M + nt - 1) // nt * nt
+    P = len(parts)
+    # behind the 256-byte epoch head: [partition][token block][k16 step][k half][row / 8][row % 8][8 channels]
+    op = k.workspace[256:256 + P * rows * K * 2].view(dt).view(P, rows // nt, K // 16, 2, nt // 8, 8, 8)
+    op = op.permute(0, 1, 4, 5, 2, 3, 6).reshape(P, rows, K)
+    for p in range(P):
+        ref = torch.ops.rotation.rotate(x, L.pairs[p], L.theta[p], L.channel_scales[p], G)
+        assert torch.equal(op[p, :M].view(torch.int16), ref.view(torch.int16)), p
+        assert not op[p, M:].view(torch.int16).any(), p
