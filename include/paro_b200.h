@@ -192,6 +192,26 @@ size_t paro_chain_workspace_bytes(const paro_chain_step *steps, int32_t n_steps,
 int paro_chain_forward(const paro_chain_step *steps, int32_t n_steps, int64_t M, void *workspace,
                        size_t workspace_bytes, paro_stream_t stream);
 
+/* ---- prefill chains: the same step descriptors for any M >= 1 (prefill chunks, more than 16 sequences in flight) --------
+ * Every step is the M > 16 path of paro_linear_forward -- the rotation pre-pass, then the INT4 wgmma GEMM -- with the step's
+ * x op in the pre-pass and its epilogue in the GEMM (paroquant_b200/csrc/paro_gemm.cu).  Each step computes what the decode
+ * chain computes: SILU_MUL is paro_debug_silu_mul's operand bit for bit; RMSNORM is T(T(h * rstd) * w) with rstd =
+ * rsqrtf(sum(h^2) / K + eps) of the previous step's residual_out; STORE gives y = T(acc), then + bias in T; ADD_RESIDUAL
+ * stores t = T(acc) (+ bias in T) to y where y is given and h = T(t + residual_in) to residual_out.  Output row m depends only
+ * on the inputs' row m, in a fixed summation order (the RMSNorm statistics too): results are bit-reproducible and do not
+ * depend on the other rows of the batch.  Checks and messages are the decode chain's; steps with tp->world > 1 give
+ * PARO_EUNSUPPORTED.  2 x n_steps launches (paro_last_launch_count()); CUDA-graph safe; no allocation, no host
+ * synchronisation.
+ * Workspace bytes for paro_prefill_chain_forward (0 on an invalid chain): pure scratch, nothing persists between calls --
+ * the rotated operand of the largest step, fp32 row statistics of every ADD_RESIDUAL step an RMSNORM step consumes, and the
+ * outputs of consumed STORE steps without y.                                                                             */
+size_t paro_prefill_chain_workspace_bytes(const paro_chain_step *steps, int32_t n_steps, int64_t M);
+
+/* Run the chain for M >= 1 rows; workspace 256-byte aligned, below paro_prefill_chain_workspace_bytes gives
+ * PARO_EWORKSPACE.                                                                                                      */
+int paro_prefill_chain_forward(const paro_chain_step *steps, int32_t n_steps, int64_t M, void *workspace,
+                               size_t workspace_bytes, paro_stream_t stream);
+
 /* ---- MoE expert block for decode batches: the routed experts of one block in TWO launches, routing read on the device ----
  * Replaces the reference's RotateSwitchGLU (paroquant/inference/backends/mlx/modules.py:159-212) on the expert format of
  * paroquant/cli/convert.py:281-406: every expert is a merged gate|up linear and a down linear, and all experts share ONE

@@ -104,6 +104,10 @@ def lib() -> ctypes.CDLL:
         L.paro_chain_workspace_bytes.argtypes = [ctypes.POINTER(ParoChainStep), i32, i64]
         L.paro_chain_forward.restype = ctypes.c_int
         L.paro_chain_forward.argtypes = [ctypes.POINTER(ParoChainStep), i32, i64, vp, sz, vp]
+        L.paro_prefill_chain_workspace_bytes.restype = sz
+        L.paro_prefill_chain_workspace_bytes.argtypes = [ctypes.POINTER(ParoChainStep), i32, i64]
+        L.paro_prefill_chain_forward.restype = ctypes.c_int
+        L.paro_prefill_chain_forward.argtypes = [ctypes.POINTER(ParoChainStep), i32, i64, vp, sz, vp]
         L.paro_tp_slot_bytes.restype = sz
         L.paro_tp_slot_bytes.argtypes = [shp, i64, i32]
         L.paro_debug_stream_plan.restype = ctypes.c_int
@@ -137,6 +141,7 @@ EXPORTED_SYMBOLS = (
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
     "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan", "paro_debug_silu_mul",
     "paro_moe_grouped_workspace_bytes", "paro_moe_grouped_forward", "paro_debug_moe_grouped_plan",
+    "paro_prefill_chain_workspace_bytes", "paro_prefill_chain_forward",
 )
 
 
@@ -356,6 +361,21 @@ def chain_forward(steps, n: int, M: int, workspace: torch.Tensor) -> None:
     with torch.cuda.device(dev):
         rc = lib().paro_chain_forward(steps, n, M, workspace.data_ptr(), workspace.numel(), _stream(dev))
     _check(rc, "chain_forward")
+
+
+def prefill_chain_workspace_bytes(steps, n: int, M: int) -> int:
+    nb = lib().paro_prefill_chain_workspace_bytes(steps, n, M)
+    if nb == 0:
+        raise RuntimeError(f"prefill_chain: {lib().paro_last_error().decode()}")
+    return nb
+
+
+def prefill_chain_forward(steps, n: int, M: int, workspace: torch.Tensor) -> None:
+    """paro_prefill_chain_forward on the current stream of the workspace's device (steps: ctypes array of ParoChainStep)."""
+    dev = workspace.device
+    with torch.cuda.device(dev):
+        rc = lib().paro_prefill_chain_forward(steps, n, M, workspace.data_ptr(), workspace.numel(), _stream(dev))
+    _check(rc, "prefill_chain_forward")
 
 
 def moe_workspace_bytes(desc: ParoMoEDesc, T: int, top_k: int) -> int:

@@ -217,9 +217,14 @@ int paro_debug_gemm_plan(const paro_linear_shape *shape, int64_t M, int32_t sms,
   return gemm_debug_plan(L, M, sms, out);
 }
 
-static int chain_to_host(const paro_chain_step *steps, int32_t n, int64_t M, HostStep *hs) {
+// The checks both chains share: every descriptor on its own here, the hand-offs between steps in chain_check_links.  The row
+// bound is the caller's: 16 for the decode chain's one launch, the GEMM's int row index for the prefill chain.
+static int chain_to_host(const paro_chain_step *steps, int32_t n, int64_t M, int64_t max_m, HostStep *hs) {
   if (!steps || n < 1 || n > PARO_CHAIN_MAX_STEPS) { set_error("chain: 1..%d steps supported", PARO_CHAIN_MAX_STEPS); return PARO_EINVAL; }
-  if (M < 1 || M > 16) { set_error("chain: 1 <= M <= 16 rows supported, got %lld", static_cast<long long>(M)); return PARO_EUNSUPPORTED; }
+  if (M < 1 || M > max_m) {
+    set_error("chain: 1 <= M <= %lld rows supported, got %lld", static_cast<long long>(max_m), static_cast<long long>(M));
+    return PARO_EUNSUPPORTED;
+  }
   for (int i = 0; i < n; ++i) {
     const paro_chain_step &c = steps[i];
     const char *why = "";
@@ -257,9 +262,32 @@ static int chain_to_host(const paro_chain_step *steps, int32_t n, int64_t M, Hos
   return PARO_OK;
 }
 
+// what one step hands the next: an input for every step, the statistics an RMSNORM step needs, matching widths, one dtype
+static int chain_check_links(const HostStep *hs, int n) {
+  const int dtype = hs[0].L.dtype;
+  for (int i = 0; i < n; ++i) {
+    const HostStep &h = hs[i];
+    if (h.L.dtype != dtype) { set_error("chain: every step must use the same activation dtype"); return PARO_EINVAL; }
+    const bool consumed = i + 1 < n && !hs[i + 1].x;
+    if (h.x) {
+      if (h.x_op == PARO_XOP_RMSNORM) { set_error("chain: step %d: RMSNORM needs the statistics of the previous step (x must be NULL)", i); return PARO_EUNSUPPORTED; }
+    } else {
+      if (i == 0) { set_error("chain: step 0 needs an input"); return PARO_EINVAL; }
+      const HostStep &P = hs[i - 1];
+      const int x_ld = h.x_op == PARO_XOP_SILU_MUL ? 2 * h.L.K : h.L.K;
+      if (h.x_op == PARO_XOP_RMSNORM && P.epi_op != PARO_EPI_ADD_RESIDUAL) { set_error("chain: step %d: RMSNORM follows an ADD_RESIDUAL epilogue", i); return PARO_EINVAL; }
+      if (P.L.N != x_ld) { set_error("chain: step %d produces %d columns, step %d consumes %d", i - 1, P.L.N, i, x_ld); return PARO_EINVAL; }
+    }
+    if (h.epi_op == PARO_EPI_ADD_RESIDUAL && (!h.res_in || !h.res_out)) { set_error("chain: step %d: ADD_RESIDUAL needs residual_in and residual_out", i); return PARO_EINVAL; }
+    if (h.epi_op == PARO_EPI_STORE && !h.y && !consumed) { set_error("chain: step %d has no output", i); return PARO_EINVAL; }
+    if (h.x_op == PARO_XOP_RMSNORM && !h.norm_w) { set_error("chain: step %d: RMSNORM needs norm_weight", i); return PARO_EINVAL; }
+  }
+  return PARO_OK;
+}
+
 size_t paro_chain_workspace_bytes(const paro_chain_step *steps, int32_t n_steps, int64_t M) {
   HostStep hs[PARO_CHAIN_MAX_STEPS] = {};
-  if (chain_to_host(steps, n_steps, M, hs) != PARO_OK) return 0;
+  if (chain_to_host(steps, n_steps, M, 16, hs) != PARO_OK) return 0;
   return stream_chain_workspace_bytes(hs, n_steps, M);
 }
 
@@ -267,10 +295,39 @@ int paro_chain_forward(const paro_chain_step *steps, int32_t n_steps, int64_t M,
                        paro_stream_t stream) {
   g_launches = 0;
   HostStep hs[PARO_CHAIN_MAX_STEPS] = {};
-  const int rc = chain_to_host(steps, n_steps, M, hs);
+  int rc = chain_to_host(steps, n_steps, M, 16, hs);
   if (rc != PARO_OK) return rc;
   if (!workspace || !aligned(workspace, 256)) { set_error("chain: workspace must be a 256-byte aligned device buffer"); return PARO_EINVAL; }
+  if ((rc = chain_check_links(hs, n_steps)) != PARO_OK) return rc;
   return stream_forward(hs, n_steps, M, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+// the prefill chain: the same descriptors for any M >= 1 (paro_gemm.cu); tensor-parallel steps stay with the decode chain
+static int prefill_chain_to_host(const paro_chain_step *steps, int32_t n, int64_t M, HostStep *hs) {
+  int rc = chain_to_host(steps, n, M, 0x7FFFFFFF, hs);
+  if (rc != PARO_OK) return rc;
+  for (int i = 0; i < n; ++i)
+    if (hs[i].tp && hs[i].tp->world > 1) {
+      set_error("prefill_chain: step %d: tensor-parallel steps run only in the decode chain (M <= 16)", i);
+      return PARO_EUNSUPPORTED;
+    }
+  return chain_check_links(hs, n);
+}
+
+size_t paro_prefill_chain_workspace_bytes(const paro_chain_step *steps, int32_t n_steps, int64_t M) {
+  HostStep hs[PARO_CHAIN_MAX_STEPS] = {};
+  if (prefill_chain_to_host(steps, n_steps, M, hs) != PARO_OK) return 0;
+  return prefill_chain_workspace_bytes(hs, n_steps, M);
+}
+
+int paro_prefill_chain_forward(const paro_chain_step *steps, int32_t n_steps, int64_t M, void *workspace, size_t workspace_bytes,
+                               paro_stream_t stream) {
+  g_launches = 0;
+  HostStep hs[PARO_CHAIN_MAX_STEPS] = {};
+  const int rc = prefill_chain_to_host(steps, n_steps, M, hs);
+  if (rc != PARO_OK) return rc;
+  if (!workspace || !aligned(workspace, 256)) { set_error("chain: workspace must be a 256-byte aligned device buffer"); return PARO_EINVAL; }
+  return prefill_chain_forward(hs, n_steps, M, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
 }
 
 size_t paro_tp_slot_bytes(const paro_linear_shape *shape, int64_t M, int32_t world) {

@@ -17,7 +17,8 @@
 //
 // The same kernel serves the MoE block's grouped GEMMs (paro_moe_grouped.cu) through its tile source: there a token block is a
 // tile slot of the routing table -- NT sorted (token, slot) rows of one expert -- the weights are that expert's, and the
-// epilogue scatters each row to its (token, slot) output row.
+// epilogue scatters each row to its (token, slot) output row.  It also serves the prefill chain (prefill_chain_forward below), whose
+// ADD_RESIDUAL steps take the residual tile source: the residual add and the next RMSNorm's row statistics in the epilogue.
 #include "paro_launch.h"
 #include "paro_tc_common.cuh"
 
@@ -44,12 +45,23 @@ struct GemmParams {
 
 // Tile source of a linear: token block tb is rows tb * NT .. tb * NT + NT - 1 of x and y, the weights are p.packed.
 struct DenseTiles {
-  static constexpr bool kGrouped = false;
+  static constexpr bool kGrouped = false, kResidual = false;
+};
+// The same tiles with a prefill chain step's ADD_RESIDUAL epilogue (paro_stream.cu finish_block's order): t = T(acc) (+ bias in T),
+// y = t where y is given, h = T(t + residual_in) -> residual_out.  With `stats`, also stats[block * M + m] = the sum of the T-rounded
+// h^2 over the block's 128 columns, for the next step's RMSNorm: per warp the thread's two columns, then a butterfly over the 8 g
+// lanes, then the 8 consumer warps in warp order through shared memory -- an order fixed by the column alone, so a row's sums do
+// not depend on NT, M or the other rows.
+struct ResidualTiles {
+  static constexpr bool kGrouped = false, kResidual = true;
+  const void *res_in;
+  void *res_out;
+  float *stats;   // [n_blocks][M] or NULL
 };
 // Tile source of a MoE block's grouped GEMM: tile slot tb is positions tb * NT .. of the routing table, all of one expert
 // (paro_moe_grouped.cu writes the table on the device).  Slots from *live_tiles on are empty and exit at once.
 struct GroupedTiles {
-  static constexpr bool kGrouped = true;
+  static constexpr bool kGrouped = true, kResidual = false;
   const int32_t *rows;          // [slots * NT]: output row (token * top_k + slot) of each position, -1 for padding
   const int32_t *tile_expert;   // [slots]
   const int32_t *live_tiles;
@@ -67,6 +79,61 @@ __device__ __forceinline__ void gemm_dequant_round(uint32_t rec, bool q2, uint32
   if (q2)   // group_size 64: channels 64..127 of the record have their own scale / zero
     d.prep(lds32(rec + kBlockScaleOff + 256 + 2 * q), lds16(rec + zero_off + 128 + q));
   d.frag(w1.x, a + 16); d.frag(w1.y, a + 20); d.frag(w1.z, a + 24); d.frag(w1.w, a + 28);
+}
+
+// ResidualTiles' epilogue for this thread's output columns n (n + 8 the other half) and its NT / 4 tokens; `red`: 8 x NT fp32 of
+// shared memory behind the barriers
+template <typename T, int NT>
+__device__ __forceinline__ void residual_epilogue(const GemmParams &p, const ResidualTiles &tiles, const float (&acc)[NT / 2], int tb, int block,
+                                                  int n, int n_end, int tile, int t, int lane, uint32_t red) {
+  T *yout = static_cast<T *>(p.y);
+  const T *rin = static_cast<const T *>(tiles.res_in);
+  T *rout = static_cast<T *>(tiles.res_out);
+  float sq[NT / 4];   // token 8j + 2t + e: h^2 of this thread's two columns
+#pragma unroll
+  for (int i = 0; i < NT / 4; ++i) sq[i] = 0.f;
+#pragma unroll
+  for (int hi = 0; hi < 2; ++hi) {
+    const int nn = n + 8 * hi;
+    if (nn >= n_end) continue;
+    const bool has_bias = p.bias != nullptr;
+    const float bias_f = has_bias ? Traits<T>::to_float(static_cast<const T *>(p.bias)[nn]) : 0.f;
+#pragma unroll
+    for (int j = 0; j < NT / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int64_t m = static_cast<int64_t>(tb) * NT + 8 * j + 2 * t + e;
+        if (m < p.M) {
+          T v = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
+          if (has_bias) v = Traits<T>::from_float(Traits<T>::to_float(v) + bias_f);
+          const int64_t o = m * p.N + nn;
+          if (yout) yout[o] = v;
+          const T h = Traits<T>::from_float(Traits<T>::to_float(v) + Traits<T>::to_float(rin[o]));
+          rout[o] = h;
+          const float hf = Traits<T>::to_float(h);
+          sq[2 * j + e] += hf * hf;
+        }
+      }
+    }
+  }
+  if (!tiles.stats) return;
+  const int g = lane >> 2;
+#pragma unroll
+  for (int i = 0; i < NT / 4; ++i) {
+    float v = sq[i];
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);   // the 8 g lanes: 16 columns of this warp
+    if (g == 0) sts_f32(red + 4 * (tile * NT + 8 * (i >> 1) + 2 * t + (i & 1)), v);
+  }
+  named_bar_sync(1, 128 * kGemmConsumers);
+  const int c = threadIdx.x - 128;   // consumer thread 0 .. 255: token c of the tile
+  const int64_t m = static_cast<int64_t>(tb) * NT + c;
+  if (c < NT && m < p.M) {
+    float s = lds_f32(red + 4 * c);
+#pragma unroll
+    for (int w = 1; w < 4 * kGemmConsumers; ++w) s += lds_f32(red + 4 * (w * NT + c));   // warp order
+    tiles.stats[static_cast<int64_t>(block) * p.M + m] = s;
+  }
 }
 
 template <typename T, int NT, typename Tiles>
@@ -192,6 +259,10 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     }
 
     // ---- epilogue: acc[4j + e] = rows r (e < 2) / r + 8, tokens 8j + 2t + (e & 1)
+    if constexpr (Tiles::kResidual) {
+      residual_epilogue<T, NT>(p, tiles, acc, tb, block, n0 + r, n_end, tile, t, lane, bars + 256);
+      return;
+    }
     T *yout = static_cast<T *>(p.y);
     const bool has_bias = p.bias != nullptr;
 #pragma unroll
@@ -257,7 +328,8 @@ size_t gemm_workspace_bytes(const Layout &L, int64_t max_m) {
 template <typename T, int NT, typename Tiles>
 static int launch_gemm(const GemmParams &p, const Tiles &tiles, cudaStream_t stream) {
   auto kern = wg_gemm_kernel<T, NT, Tiles>;
-  const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256;
+  const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256 +
+                      (Tiles::kResidual ? static_cast<size_t>(4 * kGemmConsumers) * NT * 4 : 0);   // the residual epilogue's warp sums
   PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
@@ -286,6 +358,20 @@ static void fill_weights(GemmParams &p, const Layout &L) {
   p.rec_off = static_cast<long long>(L.rec_off);
 }
 
+// a linear's GEMM over M rows in tiles of NT, x_rot (m_pad rows per partition) at xr
+static GemmParams dense_params(const Layout &L, const void *packed, const void *xr, void *y, const void *bias, int64_t M, int NT, int64_t m_pad) {
+  GemmParams p;
+  p.packed = static_cast<const uint8_t *>(packed);
+  p.xr = static_cast<const uint8_t *>(xr);
+  p.y = y;
+  p.bias = bias;
+  fill_weights(p, L);
+  p.M = static_cast<int>(M); p.NT = NT;
+  p.tok_blocks = static_cast<int>(m_pad / NT);
+  p.xr_part_stride = static_cast<long long>(m_pad) * L.K * 2;
+  return p;
+}
+
 int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
                  const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
   if (workspace_bytes < gemm_workspace_bytes(L, M)) {
@@ -295,25 +381,87 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
   const int sms = device_sms();
   const int NT = pick_nt(M, L, sms > 0 ? sms : 132);
   const int64_t m_pad = (M + NT - 1) / NT * NT;
-  const uint8_t *pk = static_cast<const uint8_t *>(packed);
-  uint8_t *xr_base = static_cast<uint8_t *>(workspace);
   // ---- pre-pass: ONE launch rotates x for every partition, output in B-operand tile order (paro_rotate.cu: rotate_small_kernel
   // fetches all stage parameters up front; the per-partition rotate_kernel launches it replaces cost 3 x ~7 us at 256 tokens)
   {
-    const int rc = rotate_small_launch(L, pk, x, xr_base, M, m_pad, NT, stream);
+    const int rc = rotate_small_launch(L, packed, x, workspace, M, m_pad, NT, stream);
     if (rc) return rc;
   }
-  GemmParams p;
-  p.packed = pk;
-  p.xr = xr_base;
-  p.y = y;
-  p.bias = bias;
-  fill_weights(p, L);
-  p.M = static_cast<int>(M); p.NT = NT;
-  p.tok_blocks = static_cast<int>(m_pad / NT);
-  p.xr_part_stride = static_cast<long long>(m_pad) * L.K * 2;
+  const GemmParams p = dense_params(L, packed, workspace, y, bias, M, NT, m_pad);
   if (s.dtype == PARO_BF16) return launch_gemm_nt<__nv_bfloat16>(p, stream);
   return launch_gemm_nt<__half>(p, stream);
+}
+
+// ------------------------------------------------------------------ prefill chain (paro_prefill_chain_forward)
+// Workspace: the rotated operand, sized for the largest step and shared by all (a step's pre-pass runs after the previous GEMM
+// is done with it), then one fp32 [blocks][M] statistics region per ADD_RESIDUAL step an RMSNORM step consumes, then the
+// output of every consumed STORE step without y.  Offsets 256-byte aligned; 0 = no region.
+struct PrefillWs {
+  size_t stats_off[PARO_CHAIN_MAX_STEPS], out_off[PARO_CHAIN_MAX_STEPS], end;
+};
+
+static PrefillWs prefill_ws(const HostStep *steps, int n, int64_t M) {
+  auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+  PrefillWs w = {};
+  size_t off = 0;
+  for (int i = 0; i < n; ++i) {
+    const size_t b = gemm_workspace_bytes(steps[i].L, M);
+    if (b > off) off = b;
+  }
+  off = up(off);
+  for (int i = 0; i < n; ++i) {
+    const HostStep &h = steps[i];
+    const bool consumed = i + 1 < n && !steps[i + 1].x;
+    if (consumed && h.epi_op == PARO_EPI_ADD_RESIDUAL && steps[i + 1].x_op == PARO_XOP_RMSNORM) {
+      w.stats_off[i] = off;
+      off += up(static_cast<size_t>(h.L.blocks_total) * M * 4);
+    }
+    if (consumed && h.epi_op == PARO_EPI_STORE && !h.y) {
+      w.out_off[i] = off;
+      off += up(static_cast<size_t>(M) * h.L.N * 2);
+    }
+  }
+  w.end = off;
+  return w;
+}
+
+size_t prefill_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) { return prefill_ws(steps, n, M).end; }
+
+// Per step two launches: the pre-pass with the step's x op as a plain launch (it reads what the previous GEMM wrote and
+// overwrites the operand that GEMM read), then the GEMM with PDL as in gemm_forward.
+int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const PrefillWs w = prefill_ws(steps, n, M);
+  if (workspace_bytes < w.end) { set_error("workspace too small: have %zu, need %zu", workspace_bytes, w.end); return PARO_EWORKSPACE; }
+  const int sms = device_sms();
+  uint8_t *ws = static_cast<uint8_t *>(workspace);
+  const void *prev_out = nullptr;
+  const float *prev_stats = nullptr;
+  int prev_blocks = 0;
+  for (int i = 0; i < n; ++i) {
+    const HostStep &h = steps[i];
+    const Layout &L = h.L;
+    const int NT = pick_nt(M, L, sms > 0 ? sms : 132);
+    const int64_t m_pad = (M + NT - 1) / NT * NT;
+    int rc = rotate_chain_launch(L, h.packed, h.x_op, h.x ? h.x : prev_out, h.norm_w, prev_stats, prev_blocks, h.eps, ws, M, m_pad, NT, stream);
+    if (rc) return rc;
+    void *y = h.y ? h.y : w.out_off[i] ? ws + w.out_off[i] : nullptr;
+    const GemmParams p = dense_params(L, h.packed, ws, y, h.bias, M, NT, m_pad);
+    const bool bf16 = L.dtype == PARO_BF16;
+    if (h.epi_op == PARO_EPI_ADD_RESIDUAL) {
+      float *stats = w.stats_off[i] ? reinterpret_cast<float *>(ws + w.stats_off[i]) : nullptr;
+      const ResidualTiles tiles = {h.res_in, h.res_out, stats};
+      rc = bf16 ? launch_gemm_nt<__nv_bfloat16>(p, stream, tiles) : launch_gemm_nt<__half>(p, stream, tiles);
+      prev_out = h.res_out;
+      prev_stats = stats;
+    } else {
+      rc = bf16 ? launch_gemm_nt<__nv_bfloat16>(p, stream) : launch_gemm_nt<__half>(p, stream);
+      prev_out = y;
+      prev_stats = nullptr;
+    }
+    if (rc) return rc;
+    prev_blocks = L.blocks_total;
+  }
+  return PARO_OK;
 }
 
 // One grouped GEMM of a MoE block (paro_moe_grouped.cu): y[rows[m], :] = x_rot[m, :] . W[expert of m's tile] for every live tile

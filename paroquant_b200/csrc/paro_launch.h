@@ -21,6 +21,10 @@ int rotate_backward_launch(const void *y, const void *gout, const void *x, const
 int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream);
 int rotate_routed_launch(const Layout &L, const void *packed, bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles,
                          int top_k, void *out, int rows_max, int nt, cudaStream_t stream);
+// the same pre-pass after a chain step's x op (PARO_XOP_*): NONE reads x [M, K]; SILU_MUL x [M, 2K] (gate | up); RMSNORM
+// h = x [M, K] with norm_w [K] and the producing step's fp32 sums of h^2, stats[b * M + m] for its 128-column blocks b < stats_blocks
+int rotate_chain_launch(const Layout &L, const void *packed, int x_op, const void *x, const void *norm_w, const float *stats, int stats_blocks,
+                        float eps, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream);
 
 // paro_prepack.cu
 int prepack_launch(const paro_linear_shape &s, const Layout &L, const int32_t *qweight, const int32_t *qzeros,
@@ -54,6 +58,9 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
                  const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int gemm_grouped_launch(const Layout &L, const void *packed, long long expert_stride, const void *xr, void *y, int NT, int slots,
                         const int32_t *rows, const int32_t *tile_expert, const int32_t *live_tiles, int dtype, cudaStream_t stream);
+// a chain for any M (paro_prefill_chain_forward): per step the pre-pass with the step's x op, then the GEMM with its epilogue
+size_t prefill_chain_workspace_bytes(const HostStep *steps, int n, int64_t M);
+int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream);
 
 // paro_moe.cu
 size_t moe_workspace_bytes(const paro_moe_desc *d, int64_t T, int32_t k);

@@ -213,7 +213,17 @@ __global__ void __launch_bounds__(128) rotate_kernel(const T *__restrict__ x, T 
 //
 // A row source says what feeds output row m: `skip(row0)` -- the block of 8 rows from row0 on is never read, leave it;
 // `padding_block(row0)` -- all 8 rows are padding, store zeros; `valid(m)` -- row m has an input (else it is a zero row);
-// `load(m, k)` -- channels k .. k + 3 of row m's input, before the channel scale.
+// `load(m, k)` -- channels k .. k + 3 of row m's input, before the channel scale; `finish(row0, k, lane, xr)` -- called once
+// per block of 8 rows by the whole warp with the loaded channels of rows row0 .. row0 + 7, before the channel scale (a no-op
+// except for RMSNorm, whose rows need the block's statistics).
+
+// SiLU * up of the [gate | up] row whose gate channel k .. k + 3 `row` points at, K channels per half -- silu_mul2, the MoE
+// decode kernel's and the decode chain's
+template <typename T>
+__device__ __forceinline__ uint2 silu_mul_load(const T *row, int K) {
+  const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + K));
+  return make_uint2(silu_mul2<T>(gate.x, up.x), silu_mul2<T>(gate.y, up.y));
+}
 
 // a linear's activations x [M, K]; rows >= M are padding
 template <typename T>
@@ -224,6 +234,36 @@ struct DenseRows {
   __device__ bool padding_block(int row0) const { return row0 >= M; }
   __device__ bool valid(int m) const { return m < M; }
   __device__ uint2 load(int m, int k) const { return *reinterpret_cast<const uint2 *>(x + static_cast<int64_t>(m) * K + k); }
+  __device__ void finish(int, int, int, uint2 (&)[8]) const {}
+};
+// a chain step's SILU_MUL x op: x [M, 2K] (gate | up)
+template <typename T>
+struct DenseSiluMulRows : DenseRows<T> {
+  __device__ uint2 load(int m, int k) const { return silu_mul_load<T>(this->x + static_cast<int64_t>(m) * (2 * this->K) + k, this->K); }
+};
+// a chain step's RMSNORM x op: h = x [M, K], norm weights w [K]; stats[b * M + m] = the producing GEMM's sum of h^2 over the
+// columns of its 128-column block b (paro_gemm.cu, ResidualTiles).  rstd of a row adds the nb partials in block order, whatever
+// the tiles, the batch or the row's neighbours, then T(T(h * rstd) * w) as the decode chain's norm2.
+template <typename T>
+struct RmsNormRows : DenseRows<T> {
+  const T *w;
+  const float *stats;
+  int nb;
+  float eps;
+  __device__ void finish(int row0, int k, int lane, uint2 (&xr)[8]) const {
+    const int m = row0 + (lane & 7);
+    float s = 0.f;
+    if (lane < 8 && m < this->M)
+      for (int b = 0; b < nb; ++b) s += __ldcg(stats + static_cast<int64_t>(b) * this->M + m);
+    const float rstd = rsqrtf(s / static_cast<float>(this->K) + eps);   // lane r: row row0 + r
+    const uint2 w2 = *reinterpret_cast<const uint2 *>(w + k);
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const float rs = __shfl_sync(0xFFFFFFFFu, rstd, r);
+      xr[r].x = norm2<T>(xr[r].x, rs, w2.x);
+      xr[r].y = norm2<T>(xr[r].y, rs, w2.y);
+    }
+  }
 };
 
 // The MoE grouped pre-passes (paro_moe_grouped.cu): output row m is routing entry rows[m] = token * top_k + slot, -1 for padding.
@@ -235,6 +275,7 @@ struct RoutedRows {
   __device__ bool skip(int row0) const { return row0 >= *live_tiles * nt; }
   __device__ bool padding_block(int row0) const { return rows[row0] < 0; }
   __device__ bool valid(int m) const { return rows[m] >= 0; }
+  __device__ void finish(int, int, int, uint2 (&)[8]) const {}
 };
 // gate_up: x [T, K], entry e reads token e / top_k
 template <typename T>
@@ -243,16 +284,12 @@ struct GatherRows : RoutedRows {
   int top_k, K;
   __device__ uint2 load(int m, int k) const { return *reinterpret_cast<const uint2 *>(x + static_cast<int64_t>(rows[m] / top_k) * K + k); }
 };
-// down: T(T(silu(gate)) * up) of h [T * top_k, 2K] (gate | up), entry e reads row e -- silu_mul2, the MoE decode kernel's
+// down: T(T(silu(gate)) * up) of h [T * top_k, 2K] (gate | up), entry e reads row e
 template <typename T>
 struct SiluMulRows : RoutedRows {
   const T *h;
   int K;
-  __device__ uint2 load(int m, int k) const {
-    const T *row = h + static_cast<int64_t>(rows[m]) * (2 * K) + k;
-    const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + K));
-    return make_uint2(silu_mul2<T>(gate.x, up.x), silu_mul2<T>(gate.y, up.y));
-  }
+  __device__ uint2 load(int m, int k) const { return silu_mul_load<T>(h + static_cast<int64_t>(rows[m]) * (2 * K) + k, K); }
 };
 
 template <typename T, typename Rows>
@@ -302,6 +339,7 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
       }
     }
     if (r0 == 0) {
+      src.finish(row0, g * G + lane * 4, lane, xr);
       // scale (one rounding, rotation.cuh:112-113), transpose into rot[channel]
       const T *ps = reinterpret_cast<const T *>(&scw);
       T v[RB][4];
@@ -361,26 +399,52 @@ __global__ void __launch_bounds__(128) rotate_small_kernel(const Rows src, T *__
   }
 }
 
-// all partitions of L in one launch, x [M, K] -> out: per partition M_store rows (a multiple of 8; rows >= M zero) in tiles of
-// `nt` tokens
-int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
+// all partitions of L in one launch, rows of `src` -> out: per partition M_store rows (a multiple of 8; rows >= M zero) in tiles
+// of `nt` tokens
+template <typename T, typename Rows>
+static int rotate_small_rows(const Layout &L, const void *packed, const Rows &src, void *out, int64_t M_store, int nt, cudaStream_t stream) {
   const int K = L.K;
   const long long tasks = static_cast<long long>(L.n_parts) * (M_store / 8) * (K / 128);
   const long long blocks = (tasks + 3) / 4;
   if (blocks > 0x7FFFFFFF) { set_error("rotate: too many rows"); return PARO_EINVAL; }
   const long long part_elems = static_cast<long long>(M_store) * K;
   const uint8_t *meta = static_cast<const uint8_t *>(packed) + L.meta_off;
-  if (L.dtype == PARO_F16)
-    rotate_small_kernel<__half><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
-        DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), K}, static_cast<__half *>(out), meta, L.meta_group_bytes,
-        part_elems, static_cast<int>(M_store), nt, K, L.krot, L.n_parts);
-  else
-    rotate_small_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(
-        DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), K}, static_cast<__nv_bfloat16 *>(out), meta,
-        L.meta_group_bytes, part_elems, static_cast<int>(M_store), nt, K, L.krot, L.n_parts);
+  rotate_small_kernel<T><<<static_cast<unsigned>(blocks), 128, 0, stream>>>(src, static_cast<T *>(out), meta, L.meta_group_bytes, part_elems,
+                                                                           static_cast<int>(M_store), nt, K, L.krot, L.n_parts);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);
   return PARO_OK;
+}
+
+int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
+  if (L.dtype == PARO_F16)
+    return rotate_small_rows<__half>(L, packed, DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), L.K}, out, M_store, nt, stream);
+  return rotate_small_rows<__nv_bfloat16>(L, packed, DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), L.K}, out,
+                                          M_store, nt, stream);
+}
+
+template <typename T>
+static int rotate_chain_T(const Layout &L, const void *packed, int x_op, const void *x, const void *norm_w, const float *stats, int stats_blocks,
+                          float eps, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
+  const DenseRows<T> dense = {static_cast<const T *>(x), static_cast<int>(M), L.K};
+  if (x_op == PARO_XOP_SILU_MUL) {
+    DenseSiluMulRows<T> r;
+    static_cast<DenseRows<T> &>(r) = dense;
+    return rotate_small_rows<T>(L, packed, r, out, M_store, nt, stream);
+  }
+  if (x_op == PARO_XOP_RMSNORM) {
+    RmsNormRows<T> r;
+    static_cast<DenseRows<T> &>(r) = dense;
+    r.w = static_cast<const T *>(norm_w); r.stats = stats; r.nb = stats_blocks; r.eps = eps;
+    return rotate_small_rows<T>(L, packed, r, out, M_store, nt, stream);
+  }
+  return rotate_small_rows<T>(L, packed, dense, out, M_store, nt, stream);
+}
+
+int rotate_chain_launch(const Layout &L, const void *packed, int x_op, const void *x, const void *norm_w, const float *stats, int stats_blocks,
+                        float eps, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
+  if (L.dtype == PARO_BF16) return rotate_chain_T<__nv_bfloat16>(L, packed, x_op, x, norm_w, stats, stats_blocks, eps, out, M, M_store, nt, stream);
+  return rotate_chain_T<__half>(L, packed, x_op, x, norm_w, stats, stats_blocks, eps, out, M, M_store, nt, stream);
 }
 
 // The pre-pass of a MoE block's grouped GEMM (paro_moe_grouped.cu): the B operand of `rows_max` routing-table positions in tiles

@@ -318,6 +318,12 @@ template <typename T> __device__ __forceinline__ uint32_t silu_mul2(uint32_t g2,
   return pack2<T>(__hmul2(Traits<T>::from_floats(a, b), unpack2<T>(u2)));
 }
 
+// RMSNorm as vLLM's (fused_add_)rms_norm: T(T(h * rstd) * w) (paro_stream.cu's RMSNORM x op and the prefill chain's pre-pass)
+template <typename T> __device__ __forceinline__ uint32_t norm2(uint32_t h2, float rstd, uint32_t w2) {
+  const float2 h = Traits<T>::to_float2(unpack2<T>(h2));
+  return pack2<T>(__hmul2(Traits<T>::from_floats(h.x * rstd, h.y * rstd), unpack2<T>(w2)));
+}
+
 template <typename T>
 __device__ __forceinline__ void sincos2(uint32_t theta_pair_bits, float &c0, float &s0, float &c1, float &s1) {
   const float2 th = Traits<T>::to_float2(unpack2<T>(theta_pair_bits));
