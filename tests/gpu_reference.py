@@ -29,12 +29,9 @@ def ulp(v: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     return torch.exp2(e - _MANT_BITS[dtype])
 
 
-def check(y: torch.Tensor, xr_parts, W: torch.Tensor, part_sizes, bias: torch.Tensor | None = None, what: str = "",
-          sum_rel: float = SUM_REL, show: int = 6) -> float:
-    """y [M, N] in T; xr_parts: the rotated activations [M, K] of every partition; W [K, N] the dequantised operand; bias [N]
-    or [M, N] in T, or None.  Raises AssertionError naming the violating elements as (row, column, 128-column block of its
-    partition, partition) with got / ref / tol; returns the largest err / tol."""
-    dt = y.dtype
+def linear_bound(xr_parts, W: torch.Tensor, part_sizes, dt: torch.dtype, bias: torch.Tensor | None = None,
+                 sum_rel: float = SUM_REL) -> tuple[torch.Tensor, torch.Tensor]:
+    """(ref, tol) of `check`: ref [M, N] in T, tol [M, N] in float64."""
     refs, mags = [], []
     n0 = 0
     for xr, n in zip(xr_parts, part_sizes):
@@ -50,6 +47,10 @@ def check(y: torch.Tensor, xr_parts, W: torch.Tensor, part_sizes, bias: torch.Te
     if bias is not None:
         ref = (ref_pre.float() + bias.float()).to(dt)
         tol = tol + ulp(ref, dt)
+    return ref, tol
+
+
+def _assert_within(y: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, part_sizes, what: str, show: int) -> float:
     y2 = y.reshape(ref.shape)
     err = (y2.double() - ref.double()).abs()
     bad = ~(err <= tol)                                       # NaN / inf in y count as violations
@@ -63,6 +64,175 @@ def check(y: torch.Tensor, xr_parts, W: torch.Tensor, part_sizes, bias: torch.Te
                          f"ref {float(ref[m, n]):.6g} tol {float(tol[m, n]):.3g}")
         raise AssertionError(f"{what}: {len(idx)} of {bad.numel()} elements outside the element-wise bound\n" + "\n".join(lines))
     return float((err / tol).max())
+
+
+def check(y: torch.Tensor, xr_parts, W: torch.Tensor, part_sizes, bias: torch.Tensor | None = None, what: str = "",
+          sum_rel: float = SUM_REL, show: int = 6) -> float:
+    """y [M, N] in T; xr_parts: the rotated activations [M, K] of every partition; W [K, N] the dequantised operand; bias [N]
+    or [M, N] in T, or None.  Raises AssertionError naming the violating elements as (row, column, 128-column block of its
+    partition, partition) with got / ref / tol; returns the largest err / tol."""
+    ref, tol = linear_bound(xr_parts, W, part_sizes, y.dtype, bias, sum_rel)
+    return _assert_within(y, ref, tol, part_sizes, what, show)
+
+
+def check_residual(h: torch.Tensor, t: tuple[torch.Tensor, torch.Tensor], r: torch.Tensor, what: str = "", show: int = 6) -> float:
+    """The residual stream h = T(t + r) [M, N] of an ADD_RESIDUAL epilogue whose linear output t is not stored.  t = (ref_t,
+    tol_t) of `linear_bound` for that linear, r the residual input in T.  t itself satisfies |t - ref_t| <= tol_t, and the
+    kernel and the reference each round t + r once to T, so every element must satisfy
+
+        |h - T(ref_t + r)| <= ulp_T(max(|h|, |T(ref_t + r)|)) + tol_t
+
+    (the ulp term is the two half-ulp roundings, taken in the larger binade when they straddle a power of two)."""
+    ref_t, tol_t = t
+    ref = (ref_t.float() + r.reshape(ref_t.shape).float()).to(h.dtype)
+    big = torch.maximum(h.reshape(ref.shape).double().abs(), ref.double().abs())
+    return _assert_within(h, ref, ulp(big, h.dtype) + tol_t, [ref.shape[1]], what, show)
+
+
+def check_residual_linear(k, L, x: torch.Tensor, h: torch.Tensor, r: torch.Tensor, bias: torch.Tensor | None = None,
+                          W: torch.Tensor | None = None, what: str = "") -> float:
+    """`check_residual` for ParoLinearKernel k (layer buffers L on the GPU) on input x: h = T(k(x, bias) + r)."""
+    t = linear_bound(rotated(L, x), k.dense_weight() if W is None else W, L.part_sizes, h.dtype, bias)
+    return check_residual(h, t, r, what)
+
+
+# ---- RMSNorm statistics
+RSTD_ULPS = 16
+
+
+def _nudge(v: torch.Tensor, ulps: int) -> torch.Tensor:
+    """fp32 v (all positive, normal) moved by `ulps` fp32 spacings."""
+    return (v.view(torch.int32) + ulps).view(torch.float32)
+
+
+def rms_operand(h: torch.Tensor, rstd: torch.Tensor, w: torch.Tensor | None) -> torch.Tensor:
+    """The RMSNORM x op for rstd [M] in fp32: T(T(h * rstd) * w) (T(h * rstd) without w), every product in fp32."""
+    n = (h.float() * rstd.float()[:, None]).to(h.dtype)
+    return n if w is None else (n.float() * w.float()).to(h.dtype)
+
+
+def rms_candidates(h: torch.Tensor, w: torch.Tensor, eps: float, ulps: int = RSTD_ULPS) -> tuple[torch.Tensor, torch.Tensor]:
+    """Every operand the RMSNORM x op can produce from h [M, K] in T: the kernel adds the fp32 h^2 in its own order and forms
+    rstd with fast division and rsqrtf, so its rstd is within a few fp32 ulps of r = fp32(1 / sqrt(mean(h^2) + eps)) (mean in
+    fp64).  The operand is a step function of rstd, so the fp32 values r - ulps .. r + ulps give every operand it can produce.
+    Returns (xs [R, K] in T, owner [R]): the distinct candidate rows and the row of h each belongs to; row m's first candidate
+    is the one of r itself (oracle.rms_norm's operand)."""
+    var = (h.double() ** 2).mean(-1)
+    r = (1.0 / torch.sqrt(var + eps)).float()
+    xs, owner = [rms_operand(h, r, w)], [torch.arange(h.shape[0], device=h.device)]
+    seen = xs[0].clone()[:, None, :]                                           # [M, distinct so far, K]
+    for i in [d for u in range(1, ulps + 1) for d in (-u, u)]:
+        xi = rms_operand(h, _nudge(r, i), w)
+        new = ~(seen == xi[:, None, :]).all(-1).any(-1)
+        if bool(new.any()):
+            rows = new.nonzero()[:, 0]
+            xs.append(xi[rows])
+            owner.append(rows)
+            seen = torch.cat([seen, torch.where(new[:, None], xi, xs[0])[:, None, :]], 1)
+    return torch.cat(xs), torch.cat(owner)
+
+
+def check_rmsnorm(y: torch.Tensor, h: torch.Tensor, w: torch.Tensor, eps: float, rotate, W: torch.Tensor, part_sizes,
+                  bias: torch.Tensor | None = None, what: str = "", show: int = 6) -> float:
+    """`check` at full strength for the output y [M, N] of an RMSNORM step on random data, where the operand depends on the
+    last fp32 bits of rstd: each row must satisfy `check`'s bound for at least one of its `rms_candidates` (h: the step's
+    input in T, the GPU's own previous stage; rotate(x) -> the rotated activations of every partition).  A wrong statistics
+    word (a missing block, a neighbour row's partial) moves rstd by far more than RSTD_ULPS and fails every candidate.
+    Raises AssertionError naming the failing rows with the elements their first candidate violates; returns, over the rows,
+    the largest of the best candidate's err / tol."""
+    xs, owner = rms_candidates(h, w, eps)
+    ref, tol = linear_bound(rotate(xs), W, part_sizes, y.dtype, bias)
+    M = y.shape[0]
+    y2 = y.reshape(M, -1)[owner]
+    ratio = ((y2.double() - ref.double()).abs() / tol).nan_to_num(nan=float("inf")).amax(-1)   # [R]
+    best = torch.full((M,), float("inf"), dtype=torch.float64, device=ratio.device).scatter_reduce(0, owner, ratio, "amin")
+    if bool((~(best <= 1.0)).any()):
+        bad = (~(best <= 1.0)).nonzero()[:, 0].tolist()
+        first = [int((owner == m).nonzero()[0, 0]) for m in bad[:show]]
+        detail = ""
+        try:
+            _assert_within(y2[first], ref[first], tol[first], part_sizes, "", show)
+        except AssertionError as e:
+            detail = str(e).split("\n", 1)[1]
+        raise AssertionError(f"{what}: {len(bad)} of {M} rows outside the element-wise bound for every rstd within "
+                             f"{RSTD_ULPS} fp32 ulps (rows {bad[:show]}); first candidate of the rows shown, as positions "
+                             f"among them:\n{detail}")
+    return float(best.max())
+
+
+def check_rmsnorm_linear(k, L, h: torch.Tensor, w: torch.Tensor, eps: float, y: torch.Tensor, bias: torch.Tensor | None = None,
+                         W: torch.Tensor | None = None, what: str = "") -> float:
+    """`check_rmsnorm` for ParoLinearKernel k (layer buffers L on the GPU): y = k(RMSNorm(h) * w)."""
+    return check_rmsnorm(y, h, w, eps, lambda x: rotated(L, x), k.dense_weight() if W is None else W, L.part_sizes, bias, what)
+
+
+# exact-statistics rows: every value is +-2^j * c with c in {1.5, 0.5} (3/8 and 5/8 of a uniform row), times COLD off the hot
+# block of an energy-concentrated row
+_COLD = 2.0 ** -3
+
+
+def exact_rms_rows(M: int, K: int, dtype: torch.dtype, seed: int, w: torch.Tensor | None = None, eps: float = 1e-8,
+                   hot=None, ulps: int = 4) -> tuple[torch.Tensor, torch.Tensor]:
+    """Residual rows h [M, K] in T (on the CPU) whose RMSNorm operand is known exactly, and that operand T(T(h * rstd) * w)
+    (T(h * rstd) without w).  Row m is +-2^j_m * c_k with 3/8 of the c 1.5 and 5/8 0.5 in a per-row permutation and signs,
+    j_m in {0, 1, 2}.  Every value is a multiple of u = 2^(j_m - 1) (2^(j_m - 4) in a hot row) and a row's sum of h^2 is below
+    2^16 u^2, so every partial sum is exact in fp32 in any order.  A uniform row (hot[m] = -1) has mean square 4^j_m exactly: rstd = 2^-j_m up to the ulps of fast
+    division and rsqrtf, and T(h * rstd) = +-c whatever those ulps.  A row with hot[m] = b keeps the scale only in 128-column
+    block b and multiplies the rest by 2^-3: block b then holds half or more of the row's energy, so any one 32-column
+    statistics word of it dropped or counted twice moves the operand (asserted here, row by row).  Every row is also asserted
+    to give the same operand for every fp32 rstd within `ulps` ulps of the fp64 value; a row that does not is drawn again.
+    hot: [M] block indices or -1; default: every third row uniform, the others hot in a seed-dependent block.
+    Values are multiples of 2^-4 below 8, so h - b is exact in T for any bias b in {+-4, +-8} (`exact_bias`)."""
+    assert K % 128 == 0
+    nb = K // 128
+    g = torch.Generator().manual_seed(seed)
+    if hot is None:
+        hot = [-1 if (m + seed) % 3 == 0 else (seed * 7 + m * 5) % nb for m in range(M)]
+    hot = [int(b) for b in hot]
+    assert len(hot) == M and all(-1 <= b < nb for b in hot)
+    base = torch.full((K,), 0.5, dtype=torch.float64)
+    base[: 3 * K // 8] = 1.5
+    rows, ops = [], []
+    wf = None if w is None else w.cpu()
+    for m in range(M):
+        for _attempt in range(20):
+            c = base[torch.randperm(K, generator=g)] * (torch.randint(0, 2, (K,), generator=g) * 2 - 1)
+            j = int(torch.randint(0, 3, (1,), generator=g))
+            v = c * 2.0 ** j
+            u = 2.0 ** (j - 1) * (_COLD if hot[m] >= 0 else 1.0)        # every value is a multiple of u
+            if hot[m] >= 0:
+                cold = torch.ones(K, dtype=torch.bool)
+                cold[128 * hot[m]:128 * hot[m] + 128] = False
+                v[cold] *= _COLD
+            h = v.to(dtype)
+            assert torch.equal(h.double(), v)
+            sq = v * v
+            s = float(sq.sum())
+            assert s < 2.0 ** 24 * u * u and torch.equal(torch.fmod(sq / (u * u), 1.0), torch.zeros(K, dtype=torch.float64))
+            r64 = 1.0 / (s / K + eps) ** 0.5
+            r = torch.tensor([r64], dtype=torch.float32)
+            x = rms_operand(h[None], r, wf)[0]
+            if not all(torch.equal(rms_operand(h[None], _nudge(r, d), wf)[0], x) for d in range(-ulps, ulps + 1)):
+                continue                                          # an operand element within `ulps` of a rounding edge
+            if hot[m] >= 0:
+                for q in range(4):                                 # one 32-column word of the hot block dropped or doubled
+                    a = 128 * hot[m] + 32 * q
+                    share = float(sq[a:a + 32].sum())
+                    for s2 in (s - share, s + share):
+                        r2 = torch.tensor([1.0 / (s2 / K + eps) ** 0.5], dtype=torch.float32)
+                        assert not torch.equal(rms_operand(h[None], r2, wf)[0], x), (m, hot[m], q)
+            rows.append(h)
+            ops.append(x)
+            break
+        else:
+            raise AssertionError(f"exact_rms_rows: row {m} found no draw whose operand is robust to {ulps} ulps of rstd")
+    return torch.stack(rows), torch.stack(ops)
+
+
+def exact_bias(N: int, seed: int, dtype: torch.dtype) -> torch.Tensor:
+    """A bias of +-4 / +-8: with h from `exact_rms_rows`, r = h - bias is exact in T and T(bias + r) = h."""
+    g = torch.Generator().manual_seed(seed)
+    return (torch.tensor([4.0, 8.0])[torch.randint(0, 2, (N,), generator=g)] * (torch.randint(0, 2, (N,), generator=g) * 2 - 1)).to(dtype)
 
 
 def rotated(L, x: torch.Tensor) -> list[torch.Tensor]:

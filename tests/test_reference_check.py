@@ -6,7 +6,8 @@ through."""
 import pytest
 import torch
 
-from gpu_reference import check, check_combine, ulp
+from gpu_reference import (_nudge, check, check_combine, check_residual, check_rmsnorm, exact_bias, exact_rms_rows, linear_bound,
+                           rms_candidates, rms_operand, ulp)
 
 M, K, PARTS = 32, 4096, [1024, 1024]
 
@@ -231,3 +232,170 @@ def test_moe_bound_flags_three_ulps_on_one_element(dt):
     assert _moe_check(c, y, exact) <= 1.0
     with pytest.raises(AssertionError, match=f"1 of 4096 elements.*\n.*token {t}, col {n}, block {n // 128}\\)"):
         _moe_check(c, bad, exact)
+
+
+# ---- the chain neighbours' bounds: the RMSNORM x op on exact-statistics rows (`exact_rms_rows` + `check`), on random data
+# (`check_rmsnorm`), and the ADD_RESIDUAL epilogue without y (`check_residual`)
+CK, CN = 2048, 256
+
+
+def _rms_case(dt, M, K=CK, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    h = (torch.randn(M, K, generator=g) * (0.5 + torch.rand(M, 1, generator=g)) * 4).to(dt)
+    h[:, torch.randperm(K, generator=g)[:K // 100]] *= 20
+    w = (1.0 + 0.1 * torch.randn(K, generator=g)).to(dt)
+    q = torch.randint(0, 16, (K, CN), generator=g) - torch.randint(0, 16, (1, CN), generator=g)
+    W = (q * 0.002 * (0.5 + torch.rand(K // 128, 1, CN, generator=g)).repeat_interleave(128, 0).view(K, -1)).to(dt)
+    return h, w, W
+
+
+def _block_stats(h, width=128):
+    """fp32 sums of h^2 per (width-column block, row), as the epilogues write them: [K / width, M]."""
+    hf = h.float()
+    return (hf * hf).view(h.shape[0], -1, width).sum(-1).t().contiguous()
+
+
+def _rstd(s, K, eps):
+    """the kernels' rstd from fp32 row sums s: rsqrt(s / K + eps) in fp32."""
+    return torch.rsqrt(s / float(K) + torch.tensor(eps, dtype=torch.float32))
+
+
+def _gpu_like_y(x, W, bias=None, chunk=64):
+    y = _fp32_chunked(x, W, chunk).to(x.dtype)
+    return y if bias is None else (y.float() + bias.float()).to(x.dtype)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+@pytest.mark.parametrize("K", [512, 5120, 8192])
+def test_exact_rows_invariants(dt, K):
+    g = torch.Generator().manual_seed(K)
+    w = (1.0 + 0.1 * torch.randn(K, generator=g)).to(dt)
+    M, nb = 12, K // 128
+    hot = [-1, 0, nb - 1, 1, -1, nb // 2, nb - 2, -1, 3 % nb, nb - 1, 2 % nb, -1]
+    h, x = exact_rms_rows(M, K, dt, seed=K, w=w, hot=hot)
+    hd = h.double() ** 2
+    exact = hd.sum(-1)
+    for order in (torch.arange(K), torch.arange(K).flip(0), torch.randperm(K, generator=g)):
+        assert torch.equal(hd[:, order].float().cumsum(-1)[:, -1].double(), exact)                      # sequential fp32
+    assert torch.equal(_block_stats(h).sum(0).double(), exact)                                          # per block, then blocks
+    assert torch.equal(_block_stats(h, 32).flip(0).cumsum(0)[-1].double(), exact)                       # per word, reversed
+    r = _rstd(exact.float(), K, 1e-8)
+    for d in range(-4, 5):
+        assert torch.equal(rms_operand(h, _nudge(r, d), w), x), d
+    for m, b in enumerate(hot):
+        if b < 0:   # uniform: mean square 4^j, T(h * rstd) = +-c exactly
+            assert set(rms_operand(h[m:m + 1], r[m:m + 1], None).abs().unique().tolist()) == {0.5, 1.5}
+            continue
+        for q in range(4):
+            a = 128 * b + 32 * q
+            share = float(hd[m, a:a + 32].sum())
+            for s2 in (exact[m] - share, exact[m] + share):
+                assert not torch.equal(rms_operand(h[m:m + 1], _rstd(s2.float()[None], K, 1e-8), w), x[m:m + 1]), (m, q)
+
+
+def test_exact_bias_keeps_rows_exact():
+    for dt in (torch.bfloat16, torch.float16):
+        h, _ = exact_rms_rows(8, 1024, dt, seed=3)
+        b = exact_bias(1024, 4, dt)
+        r = (h.double() - b.double()).to(dt)
+        assert torch.equal(r.double(), h.double() - b.double())
+        assert torch.equal((b.float() + r.float()).to(dt), h)
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_rmsnorm_bound_accepts_other_fp32_orders(dt):
+    M, eps = 64, 1e-5
+    h, w, W = _rms_case(dt, M)
+    ident = lambda x: [x]   # noqa: E731  the bound is rotation-agnostic: the CPU cases use the operand as it is
+    for width, chunk in ((128, 64), (32, 16), (CK, CK)):
+        stats = _block_stats(h, width)
+        for s in (stats.sum(0), stats.flip(0).cumsum(0)[-1]):
+            y = _gpu_like_y(rms_operand(h, _rstd(s, CK, eps), w), W, chunk=chunk)
+            assert check_rmsnorm(y, h, w, eps, ident, W, [CN]) <= 1.0
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+@pytest.mark.parametrize("with_bias", [False, True])
+def test_residual_bound_accepts_other_fp32_orders(dt, with_bias):
+    xrs, W, bias = _case(dt, seed=6)
+    b = bias if with_bias else None
+    r = (torch.randn(M, sum(PARTS), generator=torch.Generator().manual_seed(7)) * 0.5).to(dt)
+    t = linear_bound(xrs, W, PARTS, dt, b)
+    for chunk in (16, 1024):
+        y = _gpu_like_y(xrs[0], W, b, chunk)
+        assert check_residual((y.float() + r.float()).to(dt), t, r) <= 1.0
+
+
+# planted faults at M = 1000 that the whole-matrix 1e-3 lets through
+FM = 1000
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_rmsnorm_bound_flags_one_row_missing_one_block(dt):
+    eps = 1e-5
+    h, w, W = _rms_case(dt, FM, seed=8)
+    stats = _block_stats(h)
+    s = stats.sum(0)
+    ok = _gpu_like_y(rms_operand(h, _rstd(s, CK, eps), w), W)
+    s[617] -= stats[CK // 128 - 1, 617]                                   # row 617's rstd without its last block
+    bad = _gpu_like_y(rms_operand(h, _rstd(s, CK, eps), w), W)
+    ref = _exact(rms_candidates(h, w, eps)[0][:FM], W).to(dt)             # oracle.rms_norm -> fp64 linear
+    assert _rel(bad, ref) < 1e-3 and _rel(ok, ref) < 1e-3
+    assert check_rmsnorm(ok, h, w, eps, lambda x: [x], W, [CN]) <= 1.0
+    with pytest.raises(AssertionError, match=r"1 of 1000 rows .*\(rows \[617\]\)"):
+        check_rmsnorm(bad, h, w, eps, lambda x: [x], W, [CN])
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_exact_rows_flag_one_statistics_word_from_the_next_row(dt):
+    """The prefill pre-pass adds row m's block partials in block order; here row m reads block b's partial of row m + 1."""
+    K = 4096
+    nb = K // 128
+    g = torch.Generator().manual_seed(9)
+    w = (1.0 + 0.1 * torch.randn(K, generator=g)).to(dt)
+    hot = [-1 if m % 3 == 0 else (m * 5) % nb for m in range(FM)]
+    h, x = exact_rms_rows(FM, K, dt, seed=9, w=w, hot=hot)
+    q = torch.randint(0, 16, (K, CN), generator=g) - torch.randint(0, 16, (1, CN), generator=g)
+    W = (q * 0.002 * (0.5 + torch.rand(K // 128, 1, CN, generator=g)).repeat_interleave(128, 0).view(K, -1)).to(dt)
+    stats = _block_stats(h)
+    m = 400
+    s = stats.sum(0)
+    assert torch.equal(rms_operand(h, _rstd(s, K, 1e-8), w), x)
+    # the first block outside both rows' hot blocks whose partials differ enough to move the operand: a cold block, so the
+    # whole-matrix error stays small
+    for b in range(nb):
+        if b in (hot[m], hot[m + 1]):
+            continue
+        s2 = s.clone()
+        s2[m] = s[m] - stats[b, m] + stats[b, m + 1]
+        op = rms_operand(h, _rstd(s2, K, 1e-8), w)
+        if not torch.equal(op, x):
+            break
+    else:
+        raise AssertionError("no cold block moves the operand")
+    y = _gpu_like_y(op, W)
+    ref = _exact(x, W).to(dt)
+    assert _rel(y, ref) < 1e-3
+    assert check(_gpu_like_y(x, W), [x], W, [CN]) <= 1.0
+    with pytest.raises(AssertionError, match=rf"elements outside the element-wise bound\n.*\(row {m}, col"):
+        check(y, [x], W, [CN])
+
+
+@pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16])
+def test_residual_bound_flags_one_block_of_one_row(dt):
+    g = torch.Generator().manual_seed(10)
+    x = torch.randn(FM, 1024, generator=g).to(dt)
+    q = torch.randint(0, 16, (1024, CN), generator=g) - torch.randint(0, 16, (1, CN), generator=g)
+    W = (q * 0.002 * (0.5 + torch.rand(8, 1, CN, generator=g)).repeat_interleave(128, 0).view(1024, -1)).to(dt)
+    r = (torch.randn(FM, CN, generator=g) * 0.3).to(dt)
+    h = (_gpu_like_y(x, W).float() + r.float()).to(dt)
+    t = linear_bound([x], W, [CN], dt)
+    assert check_residual(h, t, r) <= 1.0
+    bad = h.clone()
+    m, b = 733, 1
+    blk = bad[m, 128 * b:128 * b + 128].double()
+    pattern = torch.tensor([4.0, -4.0], dtype=torch.float64).repeat(64)      # +-4 ulps, alternating
+    bad[m, 128 * b:128 * b + 128] = (blk + pattern * ulp(blk, dt)).to(dt)
+    assert _rel(bad, h) < 1e-3
+    with pytest.raises(AssertionError, match=rf"elements outside the element-wise bound\n.*\(row {m}, col \d+, block {b}, part 0\)"):
+        check_residual(bad, t, r)
