@@ -282,6 +282,34 @@ int paro_moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_
  * in total.  The plan does not depend on the SM count; `sms` must be >= 1.                                                */
 int paro_debug_moe_grouped_plan(const paro_moe_desc *d, int64_t T, int32_t top_k, int32_t sms, int32_t *out);
 
+/* ---- MoE router: logits, softmax and top-k of a block in ONE launch, written where the two expert-block entry points read ----
+ * For x [T, hidden] and the router weight router_w [n_experts, hidden] (row-major, as a checkpoint stores mlp.gate.weight; no
+ * prepack), both of dtype D (PARO_F16 | PARO_BF16):
+ *   logit[t, e]        = D(sum_h x[t, h] * w[e, h])          fp32 accumulation, one rounding to D
+ *   p[t, :]            = softmax(fp32(logit[t, :]))          fp32, max subtracted first
+ *   slots              = the top_k experts by descending logit; equal logits -> lower expert id first; slot 0 is the largest
+ *   topk_weights[t, s] = p[t, id_s]                          (renormalize = 0)
+ *                      = p[t, id_s] / sum_s' p[t, id_s']     (renormalize = 1, the sum taken in slot order)
+ *   topk_ids[t, s]     = id_s
+ * (softmax -> top-k -> optional renormalise, as Qwen3-MoE's norm_topk_prob and Mixtral route).  logits_or_null, when given,
+ * receives the fp32 values of the D-rounded logits, [T, n_experts].  Row t of every output depends on row t of x and on router_w
+ * only: hidden is cut into K slices fixed by hidden alone and the slice sums are added in slice order, whatever T, the row's
+ * position in the batch and the launch plan -- a token routes bit-identically in a 1-token step and inside a prefill chunk.
+ * hidden a multiple of 128, 1 <= n_experts <= 256, 1 <= top_k <= min(n_experts, 16); otherwise PARO_EUNSUPPORTED.  x and
+ * router_w 16-byte, the outputs 4-byte aligned.  T = 0 succeeds without a launch.  One launch (paro_last_launch_count() reports
+ * 1), no workspace, no allocation, no host synchronisation; CUDA-graph safe.  The kernel releases its programmatic dependents
+ * at once: paro_moe_forward's kernels, launched next in the stream, start their prologue under it and wait for its completion
+ * before they read the routing.                                                                                              */
+int paro_moe_route(const void *x, const void *router_w, int32_t dtype, int64_t T, int32_t hidden, int32_t n_experts,
+                   int32_t top_k, int32_t renormalize, int32_t *topk_ids, float *topk_weights, float *logits_or_null,
+                   paro_stream_t stream);
+
+/* Test hook (host only): the plan of paro_moe_route on a device with `sms` SMs.  out[0] = NT (tokens per tile: 8, 16 or 32),
+ * out[1] = cluster size c (1, 2, 4 or 8 CTAs per token tile), out[2] = K slices (a function of hidden alone), out[3] = grid,
+ * out[4] = shared-memory bytes, out[5] = the number of coverage violations from a walk of the plan (a (token tile, K slice)
+ * owned other than exactly once), out[6] = token tiles, out[7] = threads per CTA.  T >= 1.                                  */
+int paro_debug_moe_route_plan(int64_t T, int32_t hidden, int32_t n_experts, int32_t top_k, int32_t sms, int32_t *out);
+
 /* Debug / test aid: dequantise the prepacked weights back to a dense [K, N] matrix of
  * shape->dtype (the exact operand the GEMM consumes).                                    */
 int paro_unpack_dense(const paro_linear_shape *shape, const void *packed, void *W_out,

@@ -129,6 +129,10 @@ def lib() -> ctypes.CDLL:
         L.paro_moe_grouped_forward.argtypes = [moe, vp, vp, vp, i64, i32, vp, vp, vp, sz, vp]
         L.paro_debug_moe_grouped_plan.restype = ctypes.c_int
         L.paro_debug_moe_grouped_plan.argtypes = [moe, i64, i32, i32, ctypes.POINTER(ctypes.c_int32)]
+        L.paro_moe_route.restype = ctypes.c_int
+        L.paro_moe_route.argtypes = [vp, vp, i32, i64, i32, i32, i32, i32, vp, vp, vp, vp]
+        L.paro_debug_moe_route_plan.restype = ctypes.c_int
+        L.paro_debug_moe_route_plan.argtypes = [i64, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_int32)]
         if L.paro_abi_version() != ABI_VERSION:
             raise ImportError("libparo_b200.so ABI version mismatch")
         _lib = L
@@ -141,7 +145,7 @@ EXPORTED_SYMBOLS = (
     "paro_chain_workspace_bytes", "paro_chain_forward", "paro_debug_stream_plan", "paro_debug_stream_trace", "paro_tp_slot_bytes",
     "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan", "paro_debug_silu_mul",
     "paro_moe_grouped_workspace_bytes", "paro_moe_grouped_forward", "paro_debug_moe_grouped_plan",
-    "paro_prefill_chain_workspace_bytes", "paro_prefill_chain_forward",
+    "paro_prefill_chain_workspace_bytes", "paro_prefill_chain_forward", "paro_moe_route", "paro_debug_moe_route_plan",
 )
 
 
@@ -439,4 +443,36 @@ def _moe_call(what: str, fn, desc: ParoMoEDesc, x, topk_ids, topk_weights, h, y,
 def debug_moe_plan(desc: ParoMoEDesc, T: int, top_k: int, sms: int) -> list[int]:
     out = (ctypes.c_int32 * 18)()
     _check(lib().paro_debug_moe_plan(ctypes.byref(desc), T, top_k, sms, out), "debug_moe_plan")
+    return list(out)
+
+
+def moe_route(x: torch.Tensor, w: torch.Tensor, top_k: int, renormalize: bool, ids_out: torch.Tensor, weights_out: torch.Tensor,
+              logits_out: torch.Tensor | None = None) -> None:
+    """paro_moe_route on the current stream of x's device: x [T, hidden] and the router weight w [E, hidden] of one dtype (float16
+    or bfloat16) -> ids_out [T, top_k] int32, weights_out [T, top_k] fp32 and, when given, logits_out [T, E] fp32; all contiguous
+    on one CUDA device.  One launch, nothing allocated."""
+    if x.dtype not in (torch.float16, torch.bfloat16) or w.dtype != x.dtype:
+        raise RuntimeError(f"moe_route: x and w must share float16 or bfloat16, got {x.dtype} / {w.dtype}")
+    if ids_out.dtype != torch.int32 or weights_out.dtype != torch.float32 or (logits_out is not None and logits_out.dtype != torch.float32):
+        raise RuntimeError("moe_route: ids_out must be int32, weights_out and logits_out float32")
+    dev = _need_cuda(x, w, ids_out, weights_out, logits_out)
+    if x.dim() != 2 or w.dim() != 2 or w.size(1) != x.size(1):
+        raise RuntimeError(f"moe_route: x must be [T, hidden] and w [E, hidden], got {tuple(x.shape)} / {tuple(w.shape)}")
+    (T, H), E, k = x.shape, w.size(0), int(top_k)
+    want = {"ids_out": ((T, k), ids_out), "weights_out": ((T, k), weights_out), "logits_out": ((T, E), logits_out)}
+    for name, (shp, t) in want.items():
+        if t is not None and tuple(t.shape) != shp:
+            raise RuntimeError(f"moe_route: {name} must be {shp}, got {tuple(t.shape)}")
+    if not all(t is None or t.is_contiguous() for t in (x, w, ids_out, weights_out, logits_out)):
+        raise RuntimeError("moe_route: all tensors must be contiguous")
+    with torch.cuda.device(dev):
+        rc = lib().paro_moe_route(x.data_ptr(), w.data_ptr(), dtype_code(x.dtype), T, H, E, k, 1 if renormalize else 0, ids_out.data_ptr(),
+                                  weights_out.data_ptr(), logits_out.data_ptr() if logits_out is not None else None, _stream(dev))
+    _check(rc, "moe_route")
+
+
+def debug_moe_route_plan(T: int, hidden: int, n_experts: int, top_k: int, sms: int) -> list[int]:
+    """[NT, cluster size, K slices, grid, shared-memory bytes, coverage violations, token tiles, threads] (include/paro_b200.h)."""
+    out = (ctypes.c_int32 * 8)()
+    _check(lib().paro_debug_moe_route_plan(T, hidden, n_experts, top_k, sms, out), "debug_moe_route_plan")
     return list(out)

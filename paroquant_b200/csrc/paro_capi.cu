@@ -372,6 +372,18 @@ int paro_debug_moe_grouped_plan(const paro_moe_desc *d, int64_t T, int32_t top_k
   return moe_grouped_debug_plan(d, T, top_k, out);
 }
 
+int paro_moe_route(const void *x, const void *router_w, int32_t dtype, int64_t T, int32_t hidden, int32_t n_experts, int32_t top_k,
+                   int32_t renormalize, int32_t *topk_ids, float *topk_weights, float *logits_or_null, paro_stream_t stream) {
+  g_launches = 0;
+  return moe_route_forward(x, router_w, dtype, T, hidden, n_experts, top_k, renormalize, topk_ids, topk_weights, logits_or_null,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int paro_debug_moe_route_plan(int64_t T, int32_t hidden, int32_t n_experts, int32_t top_k, int32_t sms, int32_t *out) {
+  if (!out || sms < 1) { set_error("debug_moe_route_plan: bad arguments"); return PARO_EINVAL; }
+  return moe_route_debug_plan(T, hidden, n_experts, top_k, sms, out);
+}
+
 int paro_debug_stream_trace(unsigned long long *host_out, int32_t max_ctas) {
   if (!host_out || max_ctas <= 0) { set_error("debug_trace: bad arguments"); return PARO_EINVAL; }
   return stream_trace_read(host_out, max_ctas);

@@ -75,4 +75,9 @@ int moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *id
                         void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int moe_grouped_debug_plan(const paro_moe_desc *d, int64_t T, int32_t k, int32_t *out);
 
+// paro_moe_route.cu
+int moe_route_forward(const void *x, const void *w, int dtype, int64_t T, int hidden, int E, int k, int renormalize, int32_t *ids, float *wts,
+                      float *logits, cudaStream_t stream);
+int moe_route_debug_plan(int64_t T, int hidden, int E, int k, int sms, int32_t *out);
+
 }  // namespace paro

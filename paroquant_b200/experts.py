@@ -6,11 +6,13 @@ The reference quantises a fused expert block with ONE rotation per projection sh
 (`inference/backends/mlx/modules.py:159-212`, `RotateSwitchGLU`: rotate x, per-expert gate / up, activation, rotate, per-expert
 down).  Here every expert is two fused linears -- merged gate|up (two partitions carrying the same rotation) and down -- so an
 expert costs two launches, or ONE for decode batches (a two-step chain with SiLU*up folded into the down step).  The rotation is
-recomputed per selected expert inside the kernel (it is a prologue of a few microseconds); routing stays in torch.
+recomputed per selected expert inside the kernel (it is a prologue of a few microseconds).
 
 `decode_step(T, top_k)` runs the whole block for a decode batch in two launches with the routing read on the device
 (include/paro_b200.h: paro_moe_forward): no host synchronisation, CUDA-graph capturable with the routing changing between replays.
 `prefill_step(T, top_k)` does the same for any T as grouped wgmma GEMMs in six launches (paro_moe_grouped_forward).
+`ParoRouter` computes the routing itself (router logits, softmax, top-k) in one more launch; given to either step as `router=`,
+the step runs from the hidden state to the block output with no torch op in between (3 and 7 launches).
 """
 from __future__ import annotations
 
@@ -22,6 +24,39 @@ from . import _cabi
 from .chain import ChainStep, ParoChain
 from .checkpoint import ParoLayerBuffers, validate_pairs
 from .linear import ParoLinearKernel
+
+
+class ParoRouter:
+    """The router of one MoE block: softmax over `weight [E, hidden] @ x`, the top_k experts (equal logits: the lower id first)
+    and their probabilities, renormalised to sum to one when `renormalize` (Qwen3-MoE's norm_topk_prob; Mixtral), in one launch
+    (include/paro_b200.h: paro_moe_route).  The weight is used as the checkpoint stores `mlp.gate.weight`, cast to the block's
+    dtype.  A token's routing does not depend on the batch it is routed in."""
+
+    def __init__(self, weight: torch.Tensor, top_k: int, renormalize: bool = True, dtype: torch.dtype = torch.bfloat16, device="cuda"):
+        if weight.dim() != 2:
+            raise RuntimeError(f"ParoRouter: weight must be [n_experts, hidden], got {tuple(weight.shape)}")
+        if dtype not in (torch.float16, torch.bfloat16):
+            raise RuntimeError(f"ParoRouter: dtype must be float16 or bfloat16, got {dtype}")
+        self.n_experts, self.hidden = weight.shape
+        self.top_k, self.renormalize, self.dtype = int(top_k), bool(renormalize), dtype
+        if self.hidden % 128 or not 1 <= self.n_experts <= 256 or not 1 <= self.top_k <= min(self.n_experts, 16):
+            raise RuntimeError(f"ParoRouter: hidden a multiple of 128, 1 <= n_experts <= 256 and 1 <= top_k <= min(n_experts, 16) supported, "
+                               f"got weight {tuple(weight.shape)}, top_k = {top_k}")
+        self.weight = weight.to(device=device, dtype=dtype).contiguous()
+
+    @classmethod
+    def from_checkpoint(cls, ck, experts_base: str, top_k: int, renormalize: bool = True, dtype: torch.dtype = torch.bfloat16,
+                        device="cuda") -> "ParoRouter":
+        """The router beside the expert block `experts_base` of a loaded checkpoint (`checkpoint_io.load_paro_checkpoint`): the
+        dense tensor `<parent of experts_base>.gate.weight`."""
+        name = experts_base.rsplit(".", 1)[0] + ".gate.weight"
+        if name not in ck.dense:
+            raise RuntimeError(f"ParoRouter: the checkpoint has no router weight {name!r} beside the expert block {experts_base!r}")
+        return cls(ck.dense[name], top_k, renormalize, dtype, device)
+
+    def __call__(self, x: torch.Tensor, ids_out: torch.Tensor, weights_out: torch.Tensor, logits_out: torch.Tensor | None = None) -> None:
+        """x [T, hidden] -> ids_out [T, top_k] int32, weights_out [T, top_k] fp32 and, when given, logits_out [T, E] fp32."""
+        _cabi.moe_route(x, self.weight, self.top_k, self.renormalize, ids_out, weights_out, logits_out)
 
 
 class ParoExperts:
@@ -109,13 +144,13 @@ class ParoExperts:
         d.down_packed, d.down_stride = self.packed["down"].data_ptr(), self.strides["down"]
         return d
 
-    def decode_step(self, T: int, top_k: int) -> "ParoMoEStep":
+    def decode_step(self, T: int, top_k: int, router: ParoRouter | None = None) -> "ParoMoEStep":
         """The block for T <= 16 tokens with top_k slots each over fixed device buffers (see ParoMoEStep)."""
-        return ParoMoEStep(self, T, top_k)
+        return ParoMoEStep(self, T, top_k, router)
 
-    def prefill_step(self, T: int, top_k: int) -> "ParoMoEPrefill":
+    def prefill_step(self, T: int, top_k: int, router: ParoRouter | None = None) -> "ParoMoEPrefill":
         """The block for any T >= 1 tokens with top_k slots each over fixed device buffers (see ParoMoEPrefill)."""
-        return ParoMoEPrefill(self, T, top_k)
+        return ParoMoEPrefill(self, T, top_k, router)
 
 
 class ParoMoEStep:
@@ -123,9 +158,11 @@ class ParoMoEStep:
     `topk_ids` [T, k] int32 and `topk_weights` [T, k] fp32 (int64 ids from torch.topk convert with a device `copy_`), call
     `step()`, read `y` [T, hidden].  `h` [T, k, 2I] holds every valid slot's gate|up output.  Construction allocates; a call
     never does, never synchronises the host, and launches two kernels on the current stream, so it can be captured in a CUDA
-    graph whose replays see whatever routing the buffers hold."""
+    graph whose replays see whatever routing the buffers hold.  With a `router`, `step()` first routes `x` on the device into
+    `topk_ids` / `topk_weights` (and the router logits into `logits` [T, E] fp32), one more launch under the same rules: only
+    `x` is an input then."""
 
-    def __init__(self, experts: ParoExperts, T: int, top_k: int):
+    def __init__(self, experts: ParoExperts, T: int, top_k: int, router: ParoRouter | None = None):
         dev = experts.packed["gate_up"].device
         self.experts, self.T, self.top_k = experts, int(T), int(top_k)
         self._desc = experts.desc()
@@ -137,8 +174,20 @@ class ParoMoEStep:
         self.h = torch.zeros(self.T, self.top_k, 2 * experts.inter, dtype=dt, device=dev)
         self.y = torch.zeros(self.T, experts.hidden, dtype=dt, device=dev)
         self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        self.router = router
+        if router is not None:
+            have = (router.n_experts, router.hidden, router.dtype, router.top_k, router.weight.device)
+            want = (experts.n_experts, experts.hidden, dt, self.top_k, dev)
+            if have != want:
+                raise RuntimeError(f"router (n_experts, hidden, dtype, top_k, device) = {have} does not match the expert block's {want}")
+            self.logits = torch.zeros(self.T, experts.n_experts, dtype=torch.float32, device=dev)
+
+    def _route(self) -> None:
+        if self.router is not None:
+            self.router(self.x, self.topk_ids, self.topk_weights, self.logits)
 
     def step(self) -> torch.Tensor:
+        self._route()
         _cabi.moe_forward(self._desc, self.x, self.topk_ids, self.topk_weights, self.h, self.y, self.workspace)
         return self.y
 
@@ -157,6 +206,7 @@ class ParoMoEPrefill(ParoMoEStep):
     _workspace_bytes = staticmethod(_cabi.moe_grouped_workspace_bytes)
 
     def step(self) -> torch.Tensor:
+        self._route()
         _cabi.moe_grouped_forward(self._desc, self.x, self.topk_ids, self.topk_weights, self.h, self.y, self.workspace)
         return self.y
 
