@@ -60,6 +60,31 @@ int device_sms() {
   return n;
 }
 
+cudaError_t smem_opt_in(const void *kernel, int bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<const void *, int>, int> granted;   // (kernel, device) -> bytes
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) {
+    std::lock_guard<std::mutex> lock(mu);
+    int &have = granted[{kernel, dev}];
+    if (have >= bytes) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) have = bytes;
+  }
+  if (e != cudaSuccess) (void)cudaGetLastError();
+  return e;
+}
+
+int ring_stages(int room, int stage_bytes, int max_stages, int multiple, int minimum, bool stages_knob) {
+  int n = room / stage_bytes;
+  if (n > max_stages) n = max_stages;
+  const int want = knobs().stages;
+  if (stages_knob && want >= multiple && want < n) n = want;
+  n = n / multiple * multiple;
+  return n < minimum ? 0 : n;
+}
+
 static bool valid_dtype(int d) { return d == PARO_F32 || d == PARO_F16 || d == PARO_BF16; }
 static bool aligned(const void *p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 

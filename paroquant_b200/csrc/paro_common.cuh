@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_90a ParoQuant kernels: dtype traits with the reference's
-// rounding points, mbarrier / bulk-copy (TMA) / PDL PTX wrappers, error plumbing.
+// Shared helpers for the sm_90a ParoQuant kernels: error plumbing and launch setup on the host (SM count, shared-memory opt-in,
+// ring depth, plan cache), dtype traits with the reference's rounding points, mbarrier / bulk-copy (TMA) / PDL PTX wrappers.
 #pragma once
 
 #include <cuda.h>
@@ -8,7 +8,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <array>
+#include <map>
+#include <mutex>
+
 #include "../../include/paro_b200.h"
+#include "paro_layout.h"
 
 namespace paro {
 
@@ -42,6 +47,48 @@ const Knobs &knobs();
 
 // SM count of the current device, asked once per device; 0 without a device
 int device_sms();
+
+// the SM count plans are made for: the device's, or an H100's 132 without a device (workspace queries then size for an H100)
+inline int planning_sms() { const int n = device_sms(); return n > 0 ? n : 132; }
+
+// Lets `kernel` use `bytes` of dynamic shared memory on the current device.  The driver is asked only when this (kernel, device)
+// has not been granted that much yet, so a grant is never lowered; a failure is returned, not remembered: the next call asks again.
+cudaError_t smem_opt_in(const void *kernel, int bytes);
+template <typename F> cudaError_t smem_opt_in(F *kernel, int bytes) { return smem_opt_in(reinterpret_cast<const void *>(kernel), bytes); }
+
+// Depth of a weight ring: the `room` bytes left after the fixed regions in stages of `stage_bytes`, at most `max_stages`, capped by
+// PARO_DECODE_STAGES if `stages_knob`, rounded down to a multiple of `multiple` (the worker sets); 0 if below `minimum`.
+int ring_stages(int room, int stage_bytes, int max_stages, int multiple, int minimum, bool stages_knob);
+
+// Rotation warps of the prologue: one per task up to 4 per set, then 8, 4, 2 until `fits(warps)` takes the carve-up (and fills it in)
+template <typename Fits> bool fit_rot_warps(int tasks, int sets, Fits fits) {
+  for (int rw = tasks < 4 * sets ? tasks : 4 * sets;; rw = rw > 8 ? 8 : rw / 2) {
+    if (fits(rw)) return true;
+    if (rw <= 2) return false;
+  }
+}
+
+// Plans that depend only on a layout's shape, M and one kernel-specific int: `search(plan)` runs once per key, its result (a
+// failure too) is looked up after that.
+template <typename Plan> struct PlanCache {
+  using Key = std::array<int, 7 + PARO_MAX_PARTS>;   // K, N, krot, qhalves, n_parts, M, extra, partition sizes
+  template <typename Search> bool get(const Layout &L, int M, int extra, Plan &out, Search search) {
+    Key k = {L.K, L.N, L.krot, L.qhalves, L.n_parts, M, extra};
+    for (int p = 0; p < L.n_parts; ++p) k[7 + p] = L.part_col_begin[p + 1] - L.part_col_begin[p];
+    std::lock_guard<std::mutex> lock(mu);
+    auto it = plans.find(k);
+    if (it == plans.end()) {
+      Entry e = {};
+      e.found = search(e.plan);
+      it = plans.emplace(k, e).first;
+    }
+    out = it->second.plan;
+    return it->second.found;
+  }
+  struct Entry { bool found; Plan plan; };
+  std::mutex mu;
+  std::map<Key, Entry> plans;
+};
 
 // cfg for `grid` CTAs of `threads` threads with `smem` bytes of dynamic shared memory; attr (cfg points at it) gets a cluster
 // dimension of `cluster` CTAs when cluster > 0 and programmatic stream serialization when pdl

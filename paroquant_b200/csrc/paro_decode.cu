@@ -23,9 +23,6 @@
 // Numerics: x_rot as paro_rotate.cu; W = T((q - z) * T(s)) with ONE rounding (the operand Marlin / AWQ
 // form); fp32 accumulation; one rounding to T; bias added in T (plugin.py:309-310).
 #include <cstdio>
-#include <cstring>
-#include <map>
-#include <mutex>
 #include <type_traits>
 
 #include "paro_launch.h"
@@ -364,12 +361,8 @@ static bool dec_carve_with(const DecPlan &plan, int M, int rot_bytes, int sets, 
   const int recv = plan.c > 1 ? ((plan.nj_max + plan.c - 1) / plan.c) * plan.c * M * 512 : 0;
   const int bar_bytes = kDecBarBytes;
   const int fixed = xb_bytes + rot_total + recv + bar_bytes + 128;
-  int nst = (kDecSmemLimit - fixed) / stage_bytes;
-  if (nst > kDecMaxStages) nst = kDecMaxStages;
-  const int want = knobs().stages;
-  if (want >= sets && want < nst) nst = want;
-  nst = nst / sets * sets;   // a stage is always consumed by the same set
-  if (nst < sets) return false;
+  const int nst = ring_stages(kDecSmemLimit - fixed, stage_bytes, kDecMaxStages, sets, sets, true);
+  if (!nst) return false;
   s.nstages = nst;
   s.rot_warps = rot_warps;
   s.xb_off = (nst * stage_bytes + 127) / 128 * 128;
@@ -382,23 +375,16 @@ static bool dec_carve_with(const DecPlan &plan, int M, int rot_bytes, int sets, 
 
 // every group gets its own rotating warp when the tiles fit; otherwise fewer warps take several groups each
 static bool dec_carve(const DecPlan &plan, int M, int rot_bytes, int sets, int stage_bytes, DecSmem &s) {
-  const int ntasks = plan.ng_max * (M > 4 ? (M + 3) / 4 : 1);
-  int rw = ntasks < 4 * sets ? ntasks : 4 * sets;
-  for (;;) {
-    if (dec_carve_with(plan, M, rot_bytes, sets, rw, stage_bytes, s)) return true;
-    if (rw <= 2) return false;
-    rw = rw > 8 ? 8 : rw / 2;
-  }
+  return fit_rot_warps(plan.ng_max * (M > 4 ? (M + 3) / 4 : 1), sets,
+                       [&](int rw) { return dec_carve_with(plan, M, rot_bytes, sets, rw, stage_bytes, s); });
 }
 
-// how many clusters of `c` CTAs with this footprint the device keeps resident (GPC granularity); cached per thread
+// how many clusters of `c` CTAs with this footprint the device keeps resident (GPC granularity); 0 when that cannot be asked
 template <typename T>
 static int max_resident_clusters(int c, int smem_bytes, int sms) {
   if (c == 1) return sms;
-  int slot = 0;
-  while ((1 << slot) < c) ++slot;
   auto kern = decode_kernel<T>;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) { (void)cudaGetLastError(); return 0; }   // never lowered: cached plans keep launching
+  if (smem_opt_in(kern, kDecSmemLimit) != cudaSuccess) return 0;
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, (sms / c) * c, 32 * (kDecWorkers + 1), smem_bytes, 0, c, false);
@@ -459,42 +445,20 @@ int decode_debug_plan(const Layout &L, int64_t M, int sets, int sms, const int32
   return PARO_OK;
 }
 
-struct DecCached { bool found; DecPlan plan; DecSmem smem; };
+struct DecCached { DecPlan plan; DecSmem smem; };
 
 // the plan (cluster size, block ranges, shared-memory carve-up) depends on the shape, M and the device only: searched once
-// (the search asks the occupancy API and sets the function attribute), then looked up -- an eager launch is a map lookup
+// (the search asks the occupancy API), then looked up -- an eager launch is a map lookup
 template <typename T>
-static DecCached dec_cached_plan(const Layout &L, int M, int sms) {
-  auto kern = decode_kernel<T>;
+static bool dec_cached_plan(const Layout &L, int M, int sms, DecCached &out) {
+  static PlanCache<DecCached> cache;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) dev = 0;
   const Knobs &kn = knobs();
-  struct Key {
-    int K, N, krot, n_parts, M, dev, qhalves, parts[PARO_MAX_PARTS];
-    bool operator<(const Key &o) const { return memcmp(this, &o, sizeof(Key)) < 0; }
-  };
-  static std::mutex mu;
-  static std::map<Key, DecCached> cache;
-  Key key;
-  memset(&key, 0, sizeof(key));
-  key.K = L.K; key.N = L.N; key.krot = L.krot; key.n_parts = L.n_parts; key.M = M; key.qhalves = L.qhalves;
-  if (cudaGetDevice(&key.dev) != cudaSuccess) key.dev = 0;
-  for (int i = 0; i < L.n_parts; ++i) key.parts[i] = L.part_col_begin[i + 1] - L.part_col_begin[i];
-  DecCached c;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    auto it = cache.find(key);
-    if (it == cache.end()) {
-      DecCached fresh = {};
-      fresh.found = dec_choose_plan(L, M, dec_rot_bytes(M), kDecSets, sms, !kn.no_cluster, kn.force_c,
-                                    [&](int cc, int smem) { return max_resident_clusters<T>(cc, smem, sms); }, fresh.plan, fresh.smem);
-      if (fresh.found && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess) {
-        (void)cudaGetLastError();
-        fresh.found = false;
-      }
-      it = cache.emplace(key, fresh).first;
-    }
-    c = it->second;
-  }
-  return c;
+  return cache.get(L, M, dev, out, [&](DecCached &c) {
+    return dec_choose_plan(L, M, dec_rot_bytes(M), kDecSets, sms, !kn.no_cluster, kn.force_c,
+                           [&](int cc, int smem) { return max_resident_clusters<T>(cc, smem, sms); }, c.plan, c.smem);
+  });
 }
 
 template <typename T>
@@ -507,6 +471,7 @@ static int launch_decode(DecParams &p, const Layout &L, const DecCached &c, cuda
     fprintf(stderr, "[paro decode] K=%d N=%d M=%d: cluster %d x %d ranges (grid %d), blocks/CTA <= %d, groups/CTA <= %d, %d stages, smem %d\n",
             L.K, L.N, p.M, best.c, best.ranges, best.grid, best.nj_max, best.ng_max, best_s.nstages, best_s.total);
 
+  PARO_CUDA_OK(smem_opt_in(kern, kDecSmemLimit));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, best.grid, 32 * (kDecWorkers + 1), best_s.total, stream, best.c > 1 ? best.c : 0, !kn.no_pdl);
@@ -545,9 +510,10 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   const int sms = device_sms();
   if (sms <= 0) { set_error("decode: no CUDA device"); return PARO_ECUDA; }
   // no plan (e.g. K too long for one CTA without clusters): the caller falls back to the stream kernel, before any launch
-  const DecCached plan = s.dtype == PARO_BF16 ? dec_cached_plan<__nv_bfloat16>(L, static_cast<int>(M), sms)
-                                              : dec_cached_plan<__half>(L, static_cast<int>(M), sms);
-  if (!plan.found) { set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, static_cast<int>(M)); return PARO_EUNSUPPORTED; }
+  DecCached plan;
+  const bool found = s.dtype == PARO_BF16 ? dec_cached_plan<__nv_bfloat16>(L, static_cast<int>(M), sms, plan)
+                                          : dec_cached_plan<__half>(L, static_cast<int>(M), sms, plan);
+  if (!found) { set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, static_cast<int>(M)); return PARO_EUNSUPPORTED; }
   const size_t part_bytes = static_cast<size_t>(kDecN) * L.K * 2;   // 16 rows (zero padded) x K of T, B-operand order
   const bool prerot = decode_wants_prerot(L, M) && scratch && scratch_bytes >= L.n_parts * part_bytes;
   if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_small_kernel)

@@ -330,7 +330,7 @@ static int launch_gemm(const GemmParams &p, const Tiles &tiles, cudaStream_t str
   auto kern = wg_gemm_kernel<T, NT, Tiles>;
   const size_t smem = static_cast<size_t>(kWStages) * kWStage + static_cast<size_t>(kBStages) * NT * 128 + 256 +
                       (Tiles::kResidual ? static_cast<size_t>(4 * kGemmConsumers) * NT * 4 : 0);   // the residual epilogue's warp sums
-  PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  PARO_CUDA_OK(smem_opt_in(kern, static_cast<int>(smem)));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, p.n_blocks * p.tok_blocks, kGemmThreads, smem, stream, 0, true);   // PDL: prologue + first weight stages overlap the pre-pass
@@ -378,8 +378,7 @@ int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed
     set_error("workspace too small: have %zu, need %zu", workspace_bytes, gemm_workspace_bytes(L, M));
     return PARO_EWORKSPACE;
   }
-  const int sms = device_sms();
-  const int NT = pick_nt(M, L, sms > 0 ? sms : 132);
+  const int NT = pick_nt(M, L, planning_sms());
   const int64_t m_pad = (M + NT - 1) / NT * NT;
   // ---- pre-pass: ONE launch rotates x for every partition, output in B-operand tile order (paro_rotate.cu: rotate_small_kernel
   // fetches all stage parameters up front; the per-partition rotate_kernel launches it replaces cost 3 x ~7 us at 256 tokens)
@@ -432,7 +431,6 @@ size_t prefill_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) { 
 int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
   const PrefillWs w = prefill_ws(steps, n, M);
   if (workspace_bytes < w.end) { set_error("workspace too small: have %zu, need %zu", workspace_bytes, w.end); return PARO_EWORKSPACE; }
-  const int sms = device_sms();
   uint8_t *ws = static_cast<uint8_t *>(workspace);
   const void *prev_out = nullptr;
   const float *prev_stats = nullptr;
@@ -440,7 +438,7 @@ int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspa
   for (int i = 0; i < n; ++i) {
     const HostStep &h = steps[i];
     const Layout &L = h.L;
-    const int NT = pick_nt(M, L, sms > 0 ? sms : 132);
+    const int NT = pick_nt(M, L, planning_sms());
     const int64_t m_pad = (M + NT - 1) / NT * NT;
     int rc = rotate_chain_launch(L, h.packed, h.x_op, h.x ? h.x : prev_out, h.norm_w, prev_stats, prev_blocks, h.eps, ws, M, m_pad, NT, stream);
     if (rc) return rc;

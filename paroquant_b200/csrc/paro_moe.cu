@@ -316,9 +316,8 @@ static bool moe_carve(const Layout &L, int T, int c, int S, MoePlan &m) {
   m.grid = m.nb * c;
   const int xb = m.ng_max * kMoeN * 256, recv = 2 * c * T * 512;
   const int fixed = xb + kMoeRotBytes + recv + kMoeTabBytes + kMoeBarBytes + 128;
-  int nst = (kMoeSmemLimit - fixed) / L.rec_bytes;
-  if (nst > kMoeMaxStages) nst = kMoeMaxStages;
-  if (nst < 4) return false;
+  const int nst = ring_stages(kMoeSmemLimit - fixed, L.rec_bytes, kMoeMaxStages, 1, 4, false);
+  if (!nst) return false;
   m.nstages = nst;
   m.xb_off = (nst * L.rec_bytes + 127) / 128 * 128;
   m.rot_off = m.xb_off + xb;
@@ -402,8 +401,7 @@ static void moe_fill(MoeParams &p, const Layout &L, const MoePlan &m, const void
 template <typename T, bool DOWN>
 static int moe_launch(const MoeParams &p, const MoePlan &m, cudaStream_t stream) {
   auto kern = moe_kernel<T, DOWN>;
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMoeSmemLimit);
-  PARO_CUDA_OK(attr_rc);
+  PARO_CUDA_OK(smem_opt_in(kern, kMoeSmemLimit));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, m.grid, kMoeThreads, m.smem, stream, m.c, true);   // a cluster launch also at c = 1
@@ -424,7 +422,7 @@ int moe_forward(const paro_moe_desc *d, const void *x, const int32_t *ids, const
     return PARO_EINVAL;
   }
   if (workspace_bytes < 256) { set_error("moe: workspace too small: have %zu, need 256", workspace_bytes); return PARO_EWORKSPACE; }
-  const int Ti = static_cast<int>(T), umax = ms.E < Ti * k ? ms.E : Ti * k, dev_sms = device_sms(), sms = dev_sms > 0 ? dev_sms : 132;
+  const int Ti = static_cast<int>(T), umax = ms.E < Ti * k ? ms.E : Ti * k, sms = planning_sms();
   MoePlan m1, m2;
   if (!moe_choose_plan(ms.gu, Ti, umax, sms, m1) || !moe_choose_plan(ms.dn, Ti, umax, sms, m2)) {
     set_error("moe: no launch configuration fits (hidden=%d, I=%d, T=%d)", ms.H, ms.I, Ti);

@@ -238,9 +238,7 @@ int moe_grouped_forward(const paro_moe_desc *d, const void *x, const int32_t *id
   uint8_t *operand = ws + gp.table_bytes, *ys = operand + gp.operand_bytes;
   const uint8_t *gu = static_cast<const uint8_t *>(d->gate_up_packed), *dn = static_cast<const uint8_t *>(d->down_packed);
 
-  static const cudaError_t attr_rc =
-      cudaFuncSetAttribute(moe_route_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRouteWarps * kGroupedMaxExperts * 4);
-  PARO_CUDA_OK(attr_rc);
+  PARO_CUDA_OK(smem_opt_in(moe_route_kernel, kRouteWarps * kGroupedMaxExperts * 4));
   moe_route_kernel<<<1, kRouteThreads, kRouteWarps * ms.E * 4, stream>>>(ids, n, ms.E, gp.nt, rows, tile_expert, live);
   PARO_CUDA_OK(cudaGetLastError());
   note_launches(1);

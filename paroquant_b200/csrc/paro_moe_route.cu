@@ -258,8 +258,7 @@ static void route_plan(int64_t T, int H, int E, int sms, RoutePlan &r) {
 template <typename T, int NB>
 static int route_launch(const RouteParams &p, const RoutePlan &r, cudaStream_t stream) {
   auto kern = moe_router_kernel<T, NB>;
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kRouteSmemLimit);
-  PARO_CUDA_OK(attr_rc);
+  PARO_CUDA_OK(smem_opt_in(kern, kRouteSmemLimit));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
   launch_config(cfg, attr, static_cast<int>(r.grid), kRouteCtaThreads, r.smem, stream, r.c, false);   // a cluster launch also at c = 1
@@ -280,9 +279,8 @@ int moe_route_forward(const void *x, const void *w, int dtype, int64_t T, int hi
     set_error("moe_route: x / router_w must be 16-byte, ids / weights / logits 4-byte aligned");
     return PARO_EINVAL;
   }
-  const int dev_sms = device_sms();
   RoutePlan r;
-  route_plan(T, hidden, E, dev_sms > 0 ? dev_sms : 132, r);
+  route_plan(T, hidden, E, planning_sms(), r);
   RouteParams p = {};
   p.x = x; p.w = w; p.ids = ids; p.wts = wts; p.logits = logits;
   p.T = T; p.H = hidden; p.E = E; p.E16 = r.e16; p.k = k; p.renorm = renormalize; p.c = r.c; p.S = r.S;

@@ -674,11 +674,11 @@ static int launch_backward_T(const void *y, const void *gout, const void *x, con
   const T *yp = static_cast<const T *>(y), *gp = static_cast<const T *>(gout), *xp = static_cast<const T *>(x);
   T *gx = static_cast<T *>(grad_x);
   if (G == 128) {
-    PARO_CUDA_OK(cudaFuncSetAttribute(rotate_backward_kernel<T, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+    PARO_CUDA_OK(smem_opt_in(rotate_backward_kernel<T, 128>, static_cast<int>(dyn)));
     rotate_backward_kernel<T, 128><<<static_cast<unsigned>(blocks), 128, dyn, stream>>>(yp, gp, xp, idx, theta, theta_dtype, scales, scales_dtype, gx, grad_theta,
                                                                                        grad_scale, M, K, krot, static_cast<int>(splits), ref_formula);
   } else {
-    PARO_CUDA_OK(cudaFuncSetAttribute(rotate_backward_kernel<T, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn)));
+    PARO_CUDA_OK(smem_opt_in(rotate_backward_kernel<T, 64>, static_cast<int>(dyn)));
     rotate_backward_kernel<T, 64><<<static_cast<unsigned>(blocks), 128, dyn, stream>>>(yp, gp, xp, idx, theta, theta_dtype, scales, scales_dtype, gx, grad_theta,
                                                                                       grad_scale, M, K, krot, static_cast<int>(splits), ref_formula);
   }

@@ -34,8 +34,6 @@
 // accumulation; one rounding to T.
 #include <cstdio>
 #include <cstring>
-#include <map>
-#include <mutex>
 #include <type_traits>
 #include <vector>
 
@@ -793,9 +791,9 @@ static bool stm_choose_plan(const Layout &L, int M, int sets, int ctas, int forc
     if (!apportion(L, pl.T, pl.part_cta_begin)) continue;   // the slice's members dealt to the partitions
     pl.ng_max = (L.groups + c - 1) / c;
     const int xb_bytes = pl.ng_max * NR * 256;
-    const int nst_room = (kStmSmemLimit - xb_bytes - 4 * sets * kGroup * 2 * stm_rot_rows(M) - kStmBarBytes - kStmMiscBytes - kStmDBufs * M * 1024 - 256) /
-                         kBlockBytesMax / sets * sets;
-    if (nst_room < sets) continue;
+    const int nst_room = ring_stages(kStmSmemLimit - xb_bytes - 4 * sets * kGroup * 2 * stm_rot_rows(M) - kStmBarBytes - kStmMiscBytes - kStmDBufs * M * 1024 - 256,
+                                     kBlockBytesMax, kStmMaxStages, sets, sets, false);
+    if (!nst_room) continue;
     pl.max_rounds = 0;
     pl.max_slots = 1;
     for (int p = 0; p < L.n_parts; ++p) {
@@ -825,23 +823,9 @@ static bool stm_choose_plan(const Layout &L, int M, int sets, int ctas, int forc
   return best_cost >= 0;
 }
 
-struct PlanKey {
-  int K, N, krot, n_parts, M, ctas, sets, parts[PARO_MAX_PARTS];
-  bool operator<(const PlanKey &o) const { return memcmp(this, &o, sizeof(PlanKey)) < 0; }
-};
-static bool stm_cached_plan(const Layout &L, int M, int sets, int ctas, StepPlan &out) {
-  static std::mutex mu;
-  static std::map<PlanKey, StepPlan> cache;
-  PlanKey k;
-  memset(&k, 0, sizeof(k));
-  k.K = L.K; k.N = L.N; k.krot = L.krot; k.n_parts = L.n_parts; k.M = M; k.ctas = ctas; k.sets = sets;
-  for (int p = 0; p < L.n_parts; ++p) k.parts[p] = L.part_col_begin[p + 1] - L.part_col_begin[p];
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = cache.find(k);
-  if (it != cache.end()) { out = it->second; return true; }
-  if (!stm_choose_plan(L, M, sets, ctas, knobs().force_c, out)) return false;
-  cache[k] = out;
-  return true;
+static bool stm_cached_plan(const Layout &L, int M, int ctas, StepPlan &out) {
+  static PlanCache<StepPlan> cache;
+  return cache.get(L, M, ctas, out, [&](StepPlan &pl) { return stm_choose_plan(L, M, kStmSets, ctas, knobs().force_c, pl); });
 }
 
 // test hook: out[0..4] = c, T, max_slots, ng_max, max_rounds; out[5..13] = part_cta_begin
@@ -878,13 +862,11 @@ bool stream_supported(const Layout &L, int64_t M) { return M >= 1 && M <= 16 && 
 // never touched by the large-M path, which keeps its scratch behind them)
 size_t stream_sync_bytes(const Layout &) { return kStmSyncBytes; }
 size_t stream_workspace_bytes(const Layout &L, int64_t max_m) {
-  const int sms = device_sms();
-  const int ctas = sms > 0 ? sms : 132;   // no device: size for an H100
   size_t need = kStmSyncBytes;
   const int top = max_m < 16 ? static_cast<int>(max_m) : 16;
   for (int M = 1; M <= top; ++M) {
     StepPlan pl;
-    if (!stm_cached_plan(L, M, kStmSets, ctas, pl)) continue;
+    if (!stm_cached_plan(L, M, planning_sms(), pl)) continue;
     const StepWs w = stm_step_ws(L, pl, M, kStmSyncBytes, false);
     if (w.end > need) need = w.end;
   }
@@ -898,38 +880,25 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
   const int M = p.M;
   p.nrows_b = stm_b_rows(M);
   p.rot_bytes = kGroup * 2 * stm_rot_rows(M);
-  const int nq = M > 4 ? (M + 3) / 4 : 1;
-  int rw = max_ng * nq < 4 * SETS ? max_ng * nq : 4 * SETS;
   const int xb_bytes = max_ng * p.nrows_b * 256;
-  for (;;) {
+  const bool fits = fit_rot_warps(max_ng * (M > 4 ? (M + 3) / 4 : 1), SETS, [&](int rw) {
     const int rot_total = (rw * p.rot_bytes + 127) / 128 * 128;
     const int fixed = xb_bytes + rot_total + kStmMiscBytes + kStmDBufs * M * 1024 + kStmBarBytes + 128;
-    int nst = (kStmSmemLimit - fixed) / p.stage_bytes;
-    if (nst > kStmMaxStages) nst = kStmMaxStages;
-    if (kn.stages >= SETS && kn.stages < nst) nst = kn.stages;
-    nst = nst / SETS * SETS;
-    if (nst >= SETS) {
-      p.nstages = nst;
-      p.inflight = kn.inflight < 1 ? 1 : kn.inflight > nst - 1 ? nst - 1 : kn.inflight;
-      p.rot_warps = rw;
-      p.xb_off = (nst * p.stage_bytes + 127) / 128 * 128;
-      p.rot_off = p.xb_off + xb_bytes;
-      p.misc_off = p.rot_off + rot_total;
-      p.dbuf_off = p.misc_off + kStmMiscBytes;
-      p.bar_off = p.dbuf_off + kStmDBufs * M * 1024;
-      break;
-    }
-    if (rw <= 2) { set_error("decode: no launch configuration fits (M=%d, %d groups per CTA)", M, max_ng); return PARO_EUNSUPPORTED; }
-    rw = rw > 8 ? 8 : rw / 2;
-  }
+    const int nst = ring_stages(kStmSmemLimit - fixed, p.stage_bytes, kStmMaxStages, SETS, SETS, true);
+    if (!nst) return false;
+    p.nstages = nst;
+    p.inflight = kn.inflight < 1 ? 1 : kn.inflight > nst - 1 ? nst - 1 : kn.inflight;
+    p.rot_warps = rw;
+    p.xb_off = (nst * p.stage_bytes + 127) / 128 * 128;
+    p.rot_off = p.xb_off + xb_bytes;
+    p.misc_off = p.rot_off + rot_total;
+    p.dbuf_off = p.misc_off + kStmMiscBytes;
+    p.bar_off = p.dbuf_off + kStmDBufs * M * 1024;
+    return true;
+  });
+  if (!fits) { set_error("decode: no launch configuration fits (M=%d, %d groups per CTA)", M, max_ng); return PARO_EUNSUPPORTED; }
   const int smem_total = p.bar_off + kStmBarBytes;
-  static thread_local bool attr_set[64] = {};   // per device: the opt-in to > 48 KB of dynamic shared memory, once
-  int dev = 0;
-  PARO_CUDA_OK(cudaGetDevice(&dev));
-  if (!attr_set[dev & 63]) {
-    PARO_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kStmSmemLimit));
-    attr_set[dev & 63] = true;
-  }
+  PARO_CUDA_OK(smem_opt_in(kern, kStmSmemLimit));
   if (kn.verbose) {
     for (int i = 0; i < p.n_steps; ++i)
       fprintf(stderr, "[paro stream] step %d K=%d N=%d M=%d: %d slices x %d members, <= %d slots/block, xop %d epi %d wait %d\n", i, p.steps[i].K,
@@ -945,12 +914,10 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
 }
 
 size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) {
-  const int sms = device_sms();
-  const int ctas = sms > 0 ? sms : 132;   // no device: size for an H100
   size_t off = kStmSyncBytes;
   for (int i = 0; i < n; ++i) {
     StepPlan pl;
-    if (!stm_cached_plan(steps[i].L, static_cast<int>(M), kStmSets, ctas, pl)) return 0;
+    if (!stm_cached_plan(steps[i].L, static_cast<int>(M), planning_sms(), pl)) return 0;
     const bool consumed = i + 1 < n && !steps[i + 1].x;
     off = stm_step_ws(steps[i].L, pl, static_cast<int>(M), off, consumed).end;
   }
@@ -975,7 +942,7 @@ int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, siz
     const HostStep &h = steps[i];
     const Layout &L = h.L;
     StepPlan pl;
-    if (!stm_cached_plan(L, p.M, kStmSets, sms, pl)) {
+    if (!stm_cached_plan(L, p.M, sms, pl)) {
       set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, p.M);
       return PARO_EUNSUPPORTED;
     }
