@@ -221,7 +221,10 @@ def c_rotate(x_f32, pairs, theta_f32, scales_f32=None, group: int = 128, dtype: 
     return from_bits(out, dtype).reshape(x.shape)
 
 
-def np_rotate(x_f32, pairs, theta_f32, scales_f32=None, group: int = 128, dtype: str = "bfloat16"):
+def np_rotate(x_f32, pairs, theta_f32, scales_f32=None, group: int = 128, dtype: str = "bfloat16", sincos=None):
+    """sincos: optional (c, s), fp32 [krot, K/2], used in place of the correctly rounded cos / sin of T(theta) -- e.g. the
+    GPU's own __sincosf values, which makes this an exact restatement of the CUDA rotation (tests/gpu_reference.py:
+    kernel_sincos).  Everything else, every rounding point included, is unchanged."""
     x, x2, th, sc, idx = _prep_rot(x_f32, pairs, theta_f32, scales_f32, dtype)
     M, K = x2.shape
     krot = idx.shape[0]
@@ -235,9 +238,13 @@ def np_rotate(x_f32, pairs, theta_f32, scales_f32=None, group: int = 128, dtype:
     for r in range(krot):
         p = idx[r].astype(np.int64).reshape(ng, group)
         pi, pj = p[:, 0::2], p[:, 1::2]                          # [ng, G/2]
-        t = th[r].astype(np.float64).reshape(ng, group // 2)
-        s_ = np.sin(t).astype(np.float32)[None]
-        c_ = np.cos(t).astype(np.float32)[None]
+        if sincos is None:
+            t = th[r].astype(np.float64).reshape(ng, group // 2)
+            s_ = np.sin(t).astype(np.float32)[None]
+            c_ = np.cos(t).astype(np.float32)[None]
+        else:
+            c_ = np.asarray(sincos[0][r], np.float32).reshape(1, ng, group // 2)
+            s_ = np.asarray(sincos[1][r], np.float32).reshape(1, ng, group // 2)
         a = _ftz(v[:, off, pi])
         b = _ftz(v[:, off, pj])
         s_b, c_b = np.broadcast_to(s_, a.shape), np.broadcast_to(c_, a.shape)

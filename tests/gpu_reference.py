@@ -1,8 +1,12 @@
 """Element-wise check of a fused linear's output against an fp64 reference (a helper module: pytest does not collect it).
 
 The fused kernels compute y[m, n] = T(sum_k x_rot[m, k] * W[k, n]) with fp32 accumulation, then add the bias in T.  The
-rotated activations (the standalone rotate kernel) and the dequantised operand (`dense_weight()`) are both checked bit for
-bit elsewhere, so what is left is the fp32 summation order and the rounding to T.  Every element must satisfy
+rotated activations (the standalone rotate kernel) and the dequantised operand (`dense_weight()`) are both pinned bit for bit:
+the rotate op equals `exact_rotate` -- oracle.np_rotate on the GPU's own sin / cos table, which is bounded against fp64 -- on
+every dtype, shape and edge value (tests/test_gpu_rotation_exact.py), and `dense_weight()` equals oracle.c_dequant at every
+shape this suite uses it for (tests/test_gpu_selection_exact.py, which also checks every fused kernel's own rotated operand
+bit for bit through selection weights).  So what is left is the fp32 summation order and the rounding to T.  Every element
+must satisfy
 
     |y - ref| <= ulp_T(ref_pre) [+ ulp_T(ref) with a bias] + 2^-16 * sum_k |x_rot[m, k] * W[k, n]|
 
@@ -236,9 +240,76 @@ def exact_bias(N: int, seed: int, dtype: torch.dtype) -> torch.Tensor:
 
 
 def rotated(L, x: torch.Tensor) -> list[torch.Tensor]:
-    """x rotated for every partition of layer buffers L (on x's device) by the standalone rotate kernel."""
+    """x rotated for every partition of layer buffers L (on x's device) by the standalone rotate kernel (equal, value for value,
+    to `exact_rotate` on every dtype, shape and edge value: tests/test_gpu_rotation_exact.py)."""
     import paroquant_b200.kernels.cuda  # noqa: F401  registers torch.ops.rotation.rotate
     return [torch.ops.rotation.rotate(x, L.pairs[p], L.theta[p], L.channel_scales[p], L.group_size) for p in range(len(L.part_sizes))]
+
+
+# ---- exact restatement of the rotation on the GPU's own sin / cos
+_ODT = {torch.float32: "float32", torch.float16: "float16", torch.bfloat16: "bfloat16"}
+# CUDA's documented maximum absolute errors for |x| <= pi (CUDA Math API, intrinsic functions): __sinf 2^-21.41, __cosf 2^-21.19
+# -- cos has the looser bound, and the H100 reaches past 2^-21.41 on it (2^-21.29 over the fp16 angles)
+SIN_ABS, COS_ABS = 2.0 ** -21.41, 2.0 ** -21.19
+
+
+def kernel_sincos(theta: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """(c, s) = __sincosf(theta) exactly as the kernels compute it, fp32 of theta's shape on the GPU.  Every kernel takes sin / cos
+    of float(theta as it reads it) -- T(theta) in the fused kernels and the half / bf16 rotate op, the raw value in the fp32 op
+    -- so pass theta already rounded to T, as fp32 values.  One fp32 rotate launch, krot = 1, no scales, identity pairs (pair t
+    of a group is channels (2t, 2t + 1)), x = 1 on every i channel and 0 on every j channel: out_i = fmaf(c, 1, s * 0) = c and
+    out_j = fmaf(c, 0, s * -1) = -s.  tests/test_gpu_rotation_exact.py bounds the table against fp64."""
+    import paroquant_b200.kernels.cuda  # noqa: F401  registers torch.ops.rotation.rotate
+    flat = theta.detach().to("cuda", torch.float32).reshape(-1)
+    n = flat.numel()
+    pad = (-n) % 64                                           # whole 128-channel groups
+    th = torch.cat([flat, flat.new_zeros(pad)])[None]
+    ch = 2 * th.shape[1]
+    x = torch.zeros(1, ch, device="cuda")
+    x[0, 0::2] = 1.0
+    pairs = (torch.arange(ch, device="cuda") % 128).to(torch.int16)[None]
+    out = torch.ops.rotation.rotate(x, pairs, th, None, 128)[0]
+    return out[0::2][:n].reshape(theta.shape), (-out[1::2][:n]).reshape(theta.shape)
+
+
+def exact_rotate(x: torch.Tensor, pairs: torch.Tensor, theta: torch.Tensor, scales: torch.Tensor | None, group: int) -> torch.Tensor:
+    """The rotate op's result for x [.., K] in T (T = x.dtype), restated on the CPU by oracle.np_rotate -- error-free fp32 FMA,
+    every rounding point of the kernels -- with the GPU's own sin / cos (`kernel_sincos` of T(theta)): the one input taken from
+    the GPU, bounded against fp64 on its own.  theta [krot, K/2] and scales [K] / [1, K] in any float dtype, read as the kernels
+    read them.  Returns x's shape and dtype on x's device."""
+    from oracle import oracle as O
+    dt = _ODT[x.dtype]
+    th = theta.detach().float().cpu().numpy()
+    c, s = kernel_sincos(torch.from_numpy(O.round_to(th, dt)))
+    sc = None if scales is None else scales.detach().float().cpu().numpy()
+    out = O.np_rotate(x.detach().float().cpu().numpy(), pairs.detach().cpu().numpy(), th, sc, group, dt,
+                      sincos=(c.cpu().numpy(), s.cpu().numpy()))
+    return torch.from_numpy(out).to(x.dtype).to(x.device)
+
+
+def exact_rotated(L, x: torch.Tensor) -> list[torch.Tensor]:
+    """`rotated` restated exactly: x [M, K] in T for every partition of layer buffers L, by `exact_rotate`."""
+    return [exact_rotate(x, L.pairs[p], L.theta[p], L.channel_scales[p], L.group_size) for p in range(len(L.part_sizes))]
+
+
+def sample_rows(M: int, block: int, seed: int, n: int = 64) -> torch.Tensor:
+    """Rows a CPU restatement looks at: all of them up to 64; above, the first 16, every row of the last `block`-row block and n
+    seeded random rows (sorted, distinct)."""
+    if M <= 64:
+        return torch.arange(M)
+    g = torch.Generator().manual_seed(seed)
+    last = torch.arange((M - 1) // block * block, M)
+    return torch.unique(torch.cat([torch.arange(16), last, torch.randint(0, M, (n,), generator=g)]))
+
+
+def assert_same_values(got: torch.Tensor, ref: torch.Tensor, what: str = "", show: int = 6) -> None:
+    """got == ref as values: +0 == -0, NaN where and only where ref has NaN, inf as inf; nothing else may differ."""
+    g, r = got.reshape(ref.shape), ref
+    same = (g == r) | (torch.isnan(g) & torch.isnan(r))
+    if not bool(same.all()):
+        idx = (~same).nonzero().tolist()
+        lines = [f"  {tuple(i)}: got {float(g[tuple(i)])!r} ref {float(r[tuple(i)])!r}" for i in idx[:show]]
+        raise AssertionError(f"{what}: {len(idx)} of {same.numel()} elements differ\n" + "\n".join(lines))
 
 
 def check_linear(k, L, x: torch.Tensor, y: torch.Tensor, bias: torch.Tensor | None = None, W: torch.Tensor | None = None,

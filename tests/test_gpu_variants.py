@@ -8,8 +8,9 @@
   * every GEMM token tile (32, 64, 128) with a ragged last tile, over 1, 2, 9 and 112 rounds of K;
   * forced plans, one child process each (the planner knobs are read once per process): every decode cluster size, the
     fall-back from decode to the stream kernel, the stream kernel at 3 and 16 K slices, in-kernel rotation up to M = 16 and
-    the pre-pass from M = 2, the GEMM for M <= 16, and the shallowest weight ring.  The parent asserts the plan the child
-    logged (PARO_DECODE_VERBOSE=1) and the number of launches, not only the numbers.
+    the pre-pass from M = 2, the GEMM for M <= 16, and the shallowest weight ring.  Every variant also runs a selection-weight
+    layer (tests/selection_layers.py), whose output must equal its exact products element for element.  The parent asserts
+    the plan the child logged (PARO_DECODE_VERBOSE=1) and the number of launches, not only the numbers.
 """
 import ctypes
 import json
@@ -275,5 +276,6 @@ def test_forced_variant(variant):
         o = obs[case["name"]]
         _expect(variant, case, o)
         plan = ", ".join(f"{k}={sorted(v)}" for k, v in sorted(o.items()) if v)
-        extra = f"max err/tol {case['ratio']:.3f}" if "ratio" in case else f"stage errors {case['stage_err']}"
+        extra = ("selection weights: every element exact" if case.get("exact") else
+                 f"max err/tol {case['ratio']:.3f}" if "ratio" in case else f"stage errors {case['stage_err']}")
         print(f"[plan] {variant}: {case['name']}: {plan}, launches {case.get('launches')}, {extra}")

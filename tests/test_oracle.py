@@ -63,6 +63,24 @@ def test_c_and_numpy_restatements_agree(oracle, dt):
 
 
 @pytest.mark.parametrize("dt", DTYPES)
+@pytest.mark.parametrize("G,krot", [(128, 8), (64, 3), (128, 16)])
+def test_np_rotate_sincos_table_of_the_default_values_is_the_default(oracle, dt, G, krot):
+    """np_rotate(sincos=(fp32(cos T(theta)), fp32(sin T(theta)))) is np_rotate bit for bit: the table replaces exactly the
+    sin / cos and nothing else.  A table of other values changes the result."""
+    L = make_synthetic_layer(512, [64], group_size=G, krot=krot, seed=11, theta_uniform_pi=True)
+    d = L.numpy_dict()
+    x = make_synthetic_activations(7, 512, dtype=torch.float32).numpy()
+    th = oracle.round_to(d["theta"][0], dt).astype(np.float64)
+    table = (np.cos(th).astype(np.float32), np.sin(th).astype(np.float32))
+    for sc in (d["channel_scales"][0], None):
+        a = oracle.np_rotate(x, d["pairs"][0], d["theta"][0], sc, G, dt)
+        b = oracle.np_rotate(x, d["pairs"][0], d["theta"][0], sc, G, dt, sincos=table)
+        assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    off = (table[0], np.nextafter(table[1], np.float32(2)) * np.float32(1.01))
+    assert not np.array_equal(a, oracle.np_rotate(x, d["pairs"][0], d["theta"][0], None, G, dt, sincos=off))
+
+
+@pytest.mark.parametrize("dt", DTYPES)
 def test_rotate_theta_zero_is_identity(oracle, dt):
     _, d = _layer()
     x = make_synthetic_activations(4, 512, dtype=torch.float32).numpy()

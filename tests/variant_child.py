@@ -6,7 +6,8 @@ tests/test_gpu_variants.py; pytest does not collect this file).
 The planner knobs (PARO_DECODE_C, PARO_NO_CLUSTER, PARO_DECODE_STREAM, PARO_DECODE_PREROT_M, PARO_SMALL_M_MAX, ...) are read
 once per process, so every variant needs its own.  The caller sets them and PARO_DECODE_VERBOSE=1: the library logs every
 launch plan on stderr, and a `[case] <name>` line on stderr before each case ties those lines to the case.  Every single
-linear is checked element-wise (gpu_reference.check_linear) and for run-to-run bit reproducibility; a decoder-tail chain is
+linear is checked element-wise (gpu_reference.check_linear) and for run-to-run bit reproducibility, a selection-weight linear
+(tests/selection_layers.py) for equality with its exact products; a decoder-tail chain is
 checked stage by stage against the single-linear entry point plus plain torch element-wise ops, normwise < 1e-3.
 """
 from __future__ import annotations
@@ -25,32 +26,44 @@ def lin(K, parts, Ms, group=128, dt="bfloat16", bias=False, krot=8, kind="linear
     return {"kind": kind, "K": K, "parts": parts, "Ms": Ms, "group": group, "dt": dt, "bias": bias, "krot": krot}
 
 
+def sel(K, parts, Ms, **kw):
+    return lin(K, parts, Ms, kind="selection", **kw)
+
+
 def tail(hidden, inter, Ms):
     return {"kind": "tail", "hidden": hidden, "inter": inter, "Ms": Ms}
 
 
-_CLUSTER_CASES = [lin(1024, [256, 128], (1, 3, 4, 9, 16), bias=True), lin(2048, [384, 128], (1, 4, 16), group=64, dt="float16", krot=9)]
+_CLUSTER_CASES = [lin(1024, [256, 128], (1, 3, 4, 9, 16), bias=True), lin(2048, [384, 128], (1, 4, 16), group=64, dt="float16", krot=9),
+                  sel(1024, [256, 128], (1, 5, 16), bias=True)]
 
 CASES = {
     # the only decode branch that stores straight to y; bias and partial last blocks included (K <= 4096: one CTA holds K)
     "decode_c1": [lin(1024, [256, 128], (1, 4, 5, 16), bias=True), lin(640, [48, 16, 32], (3, 16), group=64, dt="float16"),
-                  lin(4096, [4096], (1, 16)), lin(2048, [384], (2, 9), krot=3)],
+                  lin(4096, [4096], (1, 16)), lin(2048, [384], (2, 9), krot=3),
+                  sel(640, [48, 16, 32], (1, 4, 16), group=64, dt="float16", krot=3)],
     "decode_c2": _CLUSTER_CASES,
     "decode_c4": _CLUSTER_CASES,
     "decode_c8": _CLUSTER_CASES,
     # decode has no plan for c = 3 / 16: single linears fall back to the stream kernel with 3 / 16 K slices
     "stream_c3": [lin(1024, [256, 128], (1, 4, 16), bias=True), lin(2048, [384], (1, 9), group=64, dt="float16", krot=7),
-                  lin(4096, [4096, 1024, 1024], (1, 16)), tail(2048, 4096, (1, 16))],
+                  lin(4096, [4096, 1024, 1024], (1, 16)), tail(2048, 4096, (1, 16)),
+                  sel(1024, [256, 128], (1, 9), group=64, dt="float16", krot=7, bias=True)],
     "stream_c16": [lin(2048, [384], (1, 4, 16), bias=True), lin(4096, [4096, 1024, 1024], (1, 9), dt="float16", krot=16),
-                   tail(2048, 4096, (1, 16))],
-    "no_cluster": [lin(1024, [256, 128], (1, 16), bias=True), lin(4096, [4096], (1, 5)), lin(14336, [4096], (1, 4))],
+                   tail(2048, 4096, (1, 16)), sel(2048, [384], (1, 16), krot=16)],
+    "no_cluster": [lin(1024, [256, 128], (1, 16), bias=True), lin(4096, [4096], (1, 5)), lin(14336, [4096], (1, 4)),
+                   sel(1024, [256, 128], (1, 5, 16), bias=True)],
     "stream_only": [lin(1024, [256, 128], (1, 5, 16), bias=True), lin(4096, [4096, 1024, 1024], (1, 16)), lin(4096, [14336, 14336], (1,)),
-                    lin(14336, [4096], (1, 16)), lin(11008, [4096], (4,))],
-    "prerot_never": [lin(1024, [256, 128], (5, 9, 16), bias=True), lin(2048, [384], (16,), group=64, krot=3), lin(14336, [4096], (4, 16))],
-    "prerot_from2": [lin(1024, [256, 128], (1, 2, 3, 4), bias=True), lin(2048, [384], (2, 4), krot=9)],
-    "gemm_only": [lin(1024, [256, 128], (1, 7, 16), bias=True), lin(4096, [4096], (1, 16)), lin(640, [48, 16, 32], (3,), group=64, dt="float16")],
+                    lin(14336, [4096], (1, 16)), lin(11008, [4096], (4,)),
+                    sel(1024, [256, 128], (1, 5, 16), group=64, dt="float16", krot=9)],
+    "prerot_never": [lin(1024, [256, 128], (5, 9, 16), bias=True), lin(2048, [384], (16,), group=64, krot=3), lin(14336, [4096], (4, 16)),
+                     sel(1024, [256, 128], (5, 16), krot=3)],
+    "prerot_from2": [lin(1024, [256, 128], (1, 2, 3, 4), bias=True), lin(2048, [384], (2, 4), krot=9), sel(1024, [256, 128], (2, 3, 4), krot=9)],
+    "gemm_only": [lin(1024, [256, 128], (1, 7, 16), bias=True), lin(4096, [4096], (1, 16)), lin(640, [48, 16, 32], (3,), group=64, dt="float16"),
+                  sel(640, [48, 16, 32], (1, 16), group=64, dt="float16", bias=True)],
     "shallow_ring": [lin(1024, [256, 128], (1, 4, 8, 16), bias=True), lin(4096, [4096], (1, 8)),
-                     lin(1024, [256, 128], (1, 8, 16), bias=True, kind="chain1"), lin(4096, [4096], (1, 8), kind="chain1")],
+                     lin(1024, [256, 128], (1, 8, 16), bias=True, kind="chain1"), lin(4096, [4096], (1, 8), kind="chain1"),
+                     sel(1024, [256, 128], (1, 8, 16), bias=True)],
 }
 
 
@@ -69,6 +82,8 @@ def _run_linear(c, M, note):
     from paroquant_b200.linear import ParoLinearKernel
 
     T = getattr(torch, c["dt"])
+    if c["kind"] == "selection":
+        return _run_selection(c, M, note, T)
     L = make_synthetic_layer(c["K"], c["parts"], group_size=c["group"], krot=c["krot"], seed=c["K"] + M, device="cuda", bias=c["bias"])
     k = ParoLinearKernel.from_buffers(L, T, check_pairs=False)
     bias = None if L.bias is None else L.bias.to(T)
@@ -86,6 +101,35 @@ def _run_linear(c, M, note):
     torch.cuda.synchronize()
     note["ratio"] = check_linear(k, L, x, y, bias, what=note["name"])
     assert torch.equal(run(), y), "not bit-reproducible run to run"
+
+
+def _run_selection(c, M, note, T):
+    """Selection weights (tests/selection_layers.py): every output element equal to its exact product."""
+    import torch
+
+    from gpu_reference import assert_same_values, exact_rotated
+    from paroquant_b200 import _cabi
+    from paroquant_b200.checkpoint import make_synthetic_activations
+    from paroquant_b200.linear import ParoLinearKernel
+    from selection_layers import cover, selection_layer
+
+    launches = set()
+    for shift in cover(c["K"], sum(c["parts"])):
+        S = selection_layer(c["K"], c["parts"], group=c["group"], krot=c["krot"], seed=c["K"] + M, shift=shift, bias=c["bias"])
+        L = S.L.to("cuda")
+        k = ParoLinearKernel.from_buffers(L, T, check_pairs=False)
+        bias = None if L.bias is None else L.bias.to(T)
+        x = make_synthetic_activations(M, c["K"], seed=M + shift, device="cuda", dtype=T)
+        y = torch.full((M, sum(c["parts"])), float("nan"), dtype=T, device="cuda")
+        k.forward_into(x, y, bias)
+        launches.add(_cabi.last_launch_count())
+        ref = S.apply(exact_rotated(L, x), T)
+        if bias is not None:
+            ref = (ref.float() + bias.float()).to(T)
+        assert_same_values(y, ref, f"{note['name']} shift {shift}")
+    assert len(launches) == 1, launches
+    note["launches"] = launches.pop()
+    note["exact"] = True
 
 
 def _run_tail(c, M, note):
