@@ -208,59 +208,40 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     const int M = p.M;
     const int g = lane >> 2, t = lane & 3;
     const RoundLane lo = round_lane<kDecN>(p.q2 != 0, tile, kh, lane);
-    const uint32_t ring_end = bar_wfull + 8 * NS;
-    // a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * rec_bytes (rec_bytes is a multiple of 8)
-    const uint32_t rec_per_bar = rec_bytes / 8, rec_at_bar0 = smem0 - bar_wfull * rec_per_bar;
-    // The round loop, specialised on the token tiles (NTT) and on tracing, so that neither is a per-round branch.  Stage
-    // and parity advance by increments: `fb` is the stage's full barrier, its empty barrier sits 8 * kDecMaxStages above.
-    // Records are taken in pairs from an even stage: the ring depth is a multiple of kDecSets (even), so a pair never
-    // wraps.  A block starting at an odd stage (ng odd) takes its first record alone, an odd count its last.
+    // a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * rec_bytes (rec_bytes is a multiple of 8); the
+    // stage's empty barrier sits 8 * kDecMaxStages above its full barrier
+    const uint32_t rec_per_bar = rec_bytes / 8;
+    // The round loop (segment_rounds: one segment = one 128-column block), specialised on the token tiles (NTT) and on
+    // tracing, so that neither is a per-round branch.
     using One = std::integral_constant<int, 1>;
     using Two = std::integral_constant<int, 2>;
     auto rounds = [&](auto ntt, auto trace) {
       constexpr int NTT = decltype(ntt)::value;
       constexpr bool TRACE = decltype(trace)::value;
-      uint32_t fb = bar_wfull, par = 0;
-      int tr = 0;   // rounds of CTA 0's per-round log written
-      float acc[2][4];
-      uint32_t bx;   // this lane's ldmatrix row in the B operand of the next group
-      auto take = [&](auto nrec) {
-        constexpr int NREC = decltype(nrec)::value;
-#pragma unroll
-        for (int i = 0; i < NREC; ++i) mbar_wait(fb + 8 * i, par);
+      RingCursor rg = {bar_wfull, 0u, bar_wfull, bar_wfull + 8 * NS, 8 * kDecMaxStages, rec_per_bar, smem0 - bar_wfull * rec_per_bar, rec_bytes};
+      int tr_seen = 0, tr_done = 0;   // records of CTA 0's per-round log written
+      auto seen = [&](int n) {
         if constexpr (TRACE) {
-          if (tr == 0) DEC_TRACE(5);
+          if (tr_seen == 0) DEC_TRACE(5);
           if (blockIdx.x == 0 && warp == 0 && lane == 0)
-            for (int i = 0; i < NREC; ++i)
-              if (tr + i < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * (tr + i) + 1] = clock64() - t_entry;   // seen full
+            for (int i = 0; i < n; ++i)
+              if (tr_seen + i < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * (tr_seen + i) + 1] = clock64() - t_entry;   // seen full
+          tr_seen += n;
         }
-        mma_rounds<T, NTT, NREC, kDecN>(fb * rec_per_bar + rec_at_bar0, rec_bytes, bx, lo, acc);
-        __syncwarp();
-        if (elect_one()) {
-#pragma unroll
-          for (int i = 0; i < NREC; ++i) mbar_arrive(fb + 8 * i + 8 * kDecMaxStages);
-        }
-        if constexpr (TRACE) {
-          if (blockIdx.x == 0 && warp == 0 && lane == 0)
-            for (int i = 0; i < NREC; ++i)
-              if (tr + i < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * (tr + i) + 2] = clock64() - t_entry;   // consumed
-          tr += NREC;
-        }
-        bx += NREC * (kDecN * 256);
-        fb += 8 * NREC;
-        if (fb == ring_end) { fb = bar_wfull; par ^= 1; }
       };
-#pragma unroll 1
-      for (int j = 0; j < nj; ++j) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] = 0.f;
+      auto done = [&](int n) {
+        if constexpr (TRACE) {
+          if (blockIdx.x == 0 && warp == 0 && lane == 0)
+            for (int i = 0; i < n; ++i)
+              if (tr_done + i < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * (tr_done + i) + 2] = clock64() - t_entry;   // MMAs issued
+          tr_done += n;
+        }
+      };
+      auto seg_begin = [&](int, uint32_t &bx, int &len) {
         bx = xb + lo.x;
-        int left = ng;
-        if ((fb - bar_wfull) & 8) { take(One{}); --left; }
-        const uint32_t pairs_end = bx + (left >> 1) * (2 * kDecN * 256);   // the pair loop counts with bx
-#pragma unroll 1
-        while (bx != pairs_end) take(Two{});
-        if (left & 1) take(One{});
+        len = ng;
+      };
+      auto seg_end = [&](int j, float (&acc)[2][4]) {
         // ---- block j closed: the k-half-1 warp hands its partial to its tile's k-half-0 warp, which adds it (fixed order)
         // and stores or pushes the sum.  Two buffers by block parity: a warp writes buffer j & 1 again only after the pair
         // barrier of block j + 1, which its partner reaches after reading it.
@@ -289,7 +270,8 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
             }
           }
         }
-      }
+      };
+      segment_rounds<T, NTT, kDecN>(rg, lo, nj, seg_begin, seg_end, seen, done);
     };
     if (p.trace) {
       if (M > 8) rounds(Two{}, std::true_type{});

@@ -239,6 +239,73 @@ __device__ __forceinline__ void mma_rounds(uint32_t rec, uint32_t rec_stride, ui
   }
 }
 
+// ------------------------------------------------------------------ round loop of the small-M kernels (decode)
+// A worker warp's place in the weight ring: `fb` = full barrier of the next stage to take, its empty barrier sits `empty_off`
+// above; stage records are rec_stride apart, the record of a stage is fb * rec_per_bar + rec_at_bar0.
+struct RingCursor {
+  uint32_t fb, par, bar0, end, empty_off, rec_per_bar, rec_at_bar0, rec_stride;
+  __device__ __forceinline__ uint32_t rec() const { return fb * rec_per_bar + rec_at_bar0; }
+  __device__ __forceinline__ void advance(int n) {
+    fb += 8 * n;
+    if (fb == end) { fb = bar0; par ^= 1; }
+  }
+  __device__ __forceinline__ void release(uint32_t first, int n) const {
+    __syncwarp();
+    if (elect_one()) {
+      for (int i = 0; i < n; ++i) mbar_arrive(first + 8 * i + empty_off);
+    }
+  }
+};
+
+// The round loop of a worker warp over `nseg` segments (runs of consecutive records that go into one accumulator):
+// seg_begin(k, bx, len) gives segment k's first B row and record count, seg_end(k, acc) hands its accumulator on.  Records
+// are taken in pairs from an even stage (the ring depth is even: a pair never wraps); a segment that starts at an odd stage
+// takes its first record alone, an odd remainder its last.  The loop counts the records left in the segment.
+// seen(n) / done(n): tracing hooks after n records' full barriers were seen / their MMAs issued.
+template <typename T, int NTT, int NR, typename SegBegin, typename SegEnd, typename Seen, typename Done>
+__device__ __forceinline__ void segment_rounds(RingCursor &rg, const RoundLane &lo, int nseg, SegBegin seg_begin, SegEnd seg_end, Seen seen,
+                                               Done done) {
+  float acc[2][4];
+  uint32_t bx = 0;   // this lane's ldmatrix row of the next record
+  int left = 0;      // records of the segment not taken yet
+  auto take = [&](auto nrec) {
+    constexpr int NREC = decltype(nrec)::value;
+    for (int i = 0; i < NREC; ++i) mbar_wait(rg.fb + 8 * i, rg.par);
+    seen(NREC);
+    mma_rounds<T, NTT, NREC, NR>(rg.rec(), rg.rec_stride, bx, lo, acc);
+    rg.release(rg.fb, NREC);
+    done(NREC);
+    bx += NREC * (NR * 256);
+    rg.advance(NREC);
+    left -= NREC;
+  };
+  int k = 0;
+#pragma unroll 1
+  while (k < nseg) {
+    seg_begin(k, bx, left);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e >> 2][e & 3] = 0.f;
+    if (left > 0 && ((rg.fb - rg.bar0) & 8)) take(std::integral_constant<int, 1>{});
+    // The pair loop sits in its own branch, with the segment's close written out on both sides, on purpose.  In this shape
+    // ptxas issues a pair's two full-barrier waits back to back (no YIELD and no address add between them) and hoists all of
+    // the pair's shared-memory loads (scale / zero words, the 128-bit weight words, the first ldmatrix) right behind them,
+    // ahead of the first dequant.  A plain `for (k) { ...; while (left >= 2) take(2); ... }` of the same operations
+    // interleaves those loads with the dequant of the first k16 steps; on an H100 the per-linear M = 1 decode ran ~3.5 %
+    // slower that way (DESIGN.md section 4).
+    if (left >= 2) {
+#pragma unroll 1
+      while (left >= 2) take(std::integral_constant<int, 2>{});
+      if (left == 1) take(std::integral_constant<int, 1>{});
+      seg_end(k, acc);
+      ++k;
+    } else {
+      if (left == 1) take(std::integral_constant<int, 1>{});
+      seg_end(k, acc);
+      ++k;
+    }
+  }
+}
+
 // ------------------------------------------------------------------ in-warp rotation of one group
 // Tile `rot` = this warp's [128 channels][ROWS] elements of T, channel-major.  Lane owns pairs
 // 2*lane and 2*lane+1 of every rotation; idxw = bytes (i0, j0, i1, j1).
