@@ -33,7 +33,6 @@ namespace paro {
 constexpr int kDecMaxStages = 24;
 constexpr int kDecSets = 4;                     // worker warps = 4 x sets = 8 row tiles x 2 k halves
 constexpr int kDecWorkers = 4 * kDecSets;
-static_assert(kDecSets % 2 == 0, "the ring depth is a multiple of kDecSets; the round loop takes records in pairs that must not wrap");
 constexpr int kDecN = 16;            // B operand rows per group: token rows, zero-padded
 constexpr int kDecSmemLimit = 227 * 1024;
 constexpr int kDecBarBytes = 16 * kDecMaxStages + 256;   // ring barriers + the x-load barrier
@@ -122,11 +121,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     fetch_meta(p.packed + p.meta_off + static_cast<size_t>(mi0 + warp / nq) * p.meta_group_bytes, p.krot, lane, rm);   // flies during the barrier initialisation
 
   if (warp == kWorkers) {
-    // one barrier per lane; every worker warp consumes every ring stage
-    if (lane < NS) {
-      mbar_init(bar_wfull + 8 * lane, 1);
-      mbar_init(bar_wempty + 8 * lane, kWorkers);
-    }
+    ring_init(bar_wfull, bar_wempty, NS, kWorkers, lane);   // every worker warp consumes every ring stage
     if (lane == 0) mbar_init(bar_xload, 1);
     fence_mbar_init();
   }
@@ -140,17 +135,14 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     // ================= producer: ONE bulk copy per round (weights + scales + zeros of a (block, group), 8576 contiguous
     // bytes); nothing here depends on the previous kernel.  The whole warp runs the loop, an elected lane issues.
     const uint64_t pol = policy_evict_first();
-    int st = 0, it = 0, j = 0, gi = 0;
+    RingProducer prod = {bar_wfull, bar_wempty, smem0, rec_bytes, NS, 0, 0};
+    int j = 0, gi = 0;
 #pragma unroll 1
     for (int r = 0; r < nrounds; ++r) {
-      if (it > 0) mbar_wait(bar_wempty + 8 * st, (it - 1) & 1);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(bar_wfull + 8 * st, rec_bytes);
-        bulk_g2s(smem0 + st * rec_bytes, rec0 + (static_cast<size_t>(j) * p.groups + gi) * rec_bytes, rec_bytes, bar_wfull + 8 * st, pol);
+      // (hooks that capture the loop counters by reference change the instructions nvcc makes of this loop)
+      prod.issue([=, &p] { return rec0 + (static_cast<size_t>(j) * p.groups + gi) * rec_bytes; }, rec_bytes, pol, [=, &p] {
         if (p.trace && blockIdx.x == 0 && r < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * r] = clock64() - t_entry;
-      }
-      __syncwarp();
-      if (++st == NS) { st = 0; ++it; }
+      });
       if (++gi == ng) { gi = 0; ++j; }
     }
   } else {
@@ -208,9 +200,6 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     const int M = p.M;
     const int g = lane >> 2, t = lane & 3;
     const RoundLane lo = round_lane<kDecN>(p.q2 != 0, tile, kh, lane);
-    // a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * rec_bytes (rec_bytes is a multiple of 8); the
-    // stage's empty barrier sits 8 * kDecMaxStages above its full barrier
-    const uint32_t rec_per_bar = rec_bytes / 8;
     // The round loop (segment_rounds: one segment = one 128-column block), specialised on the token tiles (NTT) and on
     // tracing, so that neither is a per-round branch.
     using One = std::integral_constant<int, 1>;
@@ -218,7 +207,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
     auto rounds = [&](auto ntt, auto trace) {
       constexpr int NTT = decltype(ntt)::value;
       constexpr bool TRACE = decltype(trace)::value;
-      RingCursor rg = {bar_wfull, 0u, bar_wfull, bar_wfull + 8 * NS, 8 * kDecMaxStages, rec_per_bar, smem0 - bar_wfull * rec_per_bar, rec_bytes};
+      RingCursor rg = {bar_wfull, 0u, bar_wfull, bar_wfull + 8 * NS, 8 * kDecMaxStages, rec_bytes / 8, smem0 - bar_wfull * (rec_bytes / 8), rec_bytes};
       int tr_seen = 0, tr_done = 0;   // records of CTA 0's per-round log written
       auto seen = [&](int n) {
         if constexpr (TRACE) {
@@ -245,15 +234,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
         // ---- block j closed: the k-half-1 warp hands its partial to its tile's k-half-0 warp, which adds it (fixed order)
         // and stores or pushes the sum.  Two buffers by block parity: a warp writes buffer j & 1 again only after the pair
         // barrier of block j + 1, which its partner reaches after reading it.
-        const uint32_t xc = xchg + ((j & 1) * 8 + tile) * (8 * 128) + lane * 4;
-        if (kh == 1) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) sts_f32(xc + i * 128, acc[i >> 2][i & 3]);
-        }
-        named_bar_sync(4 + tile, 64);
-        if (kh == 0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] += lds_f32(xc + i * 128);
+        khalf_meet(acc, xchg + ((j & 1) * 8 + tile) * (8 * 128) + lane * 4, kh, 4 + tile, [&] {
           if (p.c > 1 && !cluster_ready) { cluster_wait_acquire(); cluster_ready = true; }  // #1: every peer CTA is running
           const uint32_t dst = p.c > 1 ? map_to_rank(recv + (((j >> p.c_shift) << p.c_shift) + slice) * (M * 512), j & (p.c - 1)) : 0u;
 #pragma unroll
@@ -269,7 +250,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
               }
             }
           }
-        }
+        });
       };
       segment_rounds<T, NTT, kDecN>(rg, lo, nj, seg_begin, seg_end, seen, done);
     };

@@ -90,10 +90,7 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
   const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
 
   if (warp == kMoeWorkers) {
-    if (lane < NS) {
-      mbar_init(bar_wfull + 8 * lane, 1);
-      mbar_init(bar_wempty + 8 * lane, kMoeWorkers);
-    }
+    ring_init(bar_wfull, bar_wempty, NS, kMoeWorkers, lane);
     fence_mbar_init();
   }
   for (int i = threadIdx.x; i < kMoeMaxEntries * 16; i += kMoeThreads) s_mask[i] = 0u;
@@ -133,7 +130,7 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
     // ================= producer: the records of my items, one bulk copy per ring stage.  It joins the cluster barrier of
     // every wave after issuing the wave's records, so it runs up to a ring ahead of the workers across waves.
     const uint64_t pol = policy_evict_first();
-    int st = 0, it = 0;
+    RingProducer prod = {bar_wfull, bar_wempty, smem0, rec_bytes, NS, 0, 0};
 #pragma unroll 1
     for (int w = 0; w < nw; ++w) {
       const int i = w * c + rank;
@@ -143,14 +140,8 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
         const uint8_t *src = p.packed + s_uexp[u] * p.stride + p.rec_off + (static_cast<size_t>(b) * G + g0) * rec_bytes;
 #pragma unroll 1
         for (int g = g0; g < g1; ++g) {
-          if (it > 0) mbar_wait(bar_wempty + 8 * st, (it - 1) & 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(bar_wfull + 8 * st, rec_bytes);
-            bulk_g2s(smem0 + st * rec_bytes, src, rec_bytes, bar_wfull + 8 * st, pol);
-          }
-          __syncwarp();
+          prod.issue([src] { return src; }, rec_bytes, pol, [] {});
           src += rec_bytes;
-          if (++st == NS) { st = 0; ++it; }
         }
       }
       cluster_wait_acquire();
@@ -164,7 +155,8 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
   const int tile = warp & 7, kh = warp >> 3;
   const int g = lane >> 2, t4 = lane & 3;
   const RoundLane lo = round_lane<kMoeN>(p.q2 != 0, tile, kh, lane);
-  uint32_t st = 0, par = 0;
+  // the ring position persists across items and waves; a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * rec_bytes
+  RingCursor rg = {bar_wfull, 0u, bar_wfull, bar_wfull + 8 * NS, 8 * kMoeMaxStages, rec_bytes / 8, smem0 - bar_wfull * (rec_bytes / 8), rec_bytes};
   const int ntok = p.T, nel = ntok * kBlockN;
   float yacc[4] = {0.f, 0.f, 0.f, 0.f}, oacc[4] = {0.f, 0.f, 0.f, 0.f};   // rank 0: elements tid + 512 q = (token, column)
   // my output columns (launch 1: gate_up has two partitions; a last partial block is masked at the stores)
@@ -172,8 +164,6 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
   const int n0 = p.part_col_begin[part] + (b - p.part_block_begin[part]) * kBlockN, n_end = p.part_col_begin[part + 1];
   cluster_wait_acquire();   // phase 0: every CTA of the cluster runs
 
-  using One = std::integral_constant<int, 1>;
-  using Two = std::integral_constant<int, 2>;
 #pragma unroll 1
   for (int w = 0; w < nw; ++w) {
     const int i = w * c + rank;
@@ -222,40 +212,25 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
         else rotation_tasks<T, 4, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
       }
       named_bar_sync(2, 32 * kMoeWorkers);   // B operand complete
-      // ---- rounds: one record per ring stage, accumulated in stream order
-      float acc[2][4];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) acc[q >> 2][q & 3] = 0.f;
-      auto rounds = [&](auto ntt) {
-        constexpr int NTT = decltype(ntt)::value;
-        uint32_t bx = xb + lo.x;
-#pragma unroll 1
-        for (int gi = 0; gi < ng; ++gi) {
-          mbar_wait(bar_wfull + 8 * st, par);
-          mma_rounds<T, NTT, 1, kMoeN>(smem0 + st * rec_bytes, rec_bytes, bx, lo, acc);
-          __syncwarp();
-          if (elect_one()) mbar_arrive(bar_wempty + 8 * st);
-          bx += kMoeN * 256;
-          if (++st == static_cast<uint32_t>(NS)) { st = 0; par ^= 1; }
-        }
+      // ---- rounds: the item is one segment of the round loop
+      auto seg_begin = [&](int, uint32_t &bx, int &len) {
+        bx = xb + lo.x;
+        len = ng;
       };
-      if (R > 8) rounds(Two{});
-      else rounds(One{});
-      // ---- k halves meet in the (now free) rotation tiles in a fixed order; the k-half-0 warp pushes the sum to rank 0
-      const uint32_t xc = rot0 + tile * (8 * 128) + lane * 4;
-      if (kh == 1) {
+      auto seg_end = [&](int, float (&acc)[2][4]) {
+        // the k halves meet in the (now free) rotation tiles in a fixed order; the k-half-0 warp pushes the sum to rank 0
+        khalf_meet(acc, rot0 + tile * (8 * 128) + lane * 4, kh, 4 + tile, [&] {
+          const uint32_t dst = map_to_rank(recv + ((w & 1) * c + rank) * (ntok * 512), 0);
 #pragma unroll
-        for (int q = 0; q < 8; ++q) sts_f32(xc + q * 128, acc[q >> 2][q & 3]);
-      }
-      named_bar_sync(4 + tile, 64);
-      if (kh == 0) {
-        const uint32_t dst = map_to_rank(recv + ((w & 1) * c + rank) * (ntok * 512), 0);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int col = 16 * tile + g + 8 * ((q >> 1) & 1), m = 8 * (q >> 2) + 2 * t4 + (q & 1);
-          if (m < R) st_cluster_f32(dst + nth_bit(tokmask, m) * 512 + col * 4, acc[q >> 2][q & 3] + lds_f32(xc + q * 128));
-        }
-      }
+          for (int q = 0; q < 8; ++q) {
+            const int col = 16 * tile + g + 8 * ((q >> 1) & 1), m = 8 * (q >> 2) + 2 * t4 + (q & 1);
+            if (m < R) st_cluster_f32(dst + nth_bit(tokmask, m) * 512 + col * 4, acc[q >> 2][q & 3]);
+          }
+        });
+      };
+      auto none = [](int) {};
+      if (R > 8) segment_rounds<T, 2, kMoeN>(rg, lo, 1, seg_begin, seg_end, none, none);
+      else segment_rounds<T, 1, kMoeN>(rg, lo, 1, seg_begin, seg_end, none, none);
     }
     cluster_arrive_release();   // my pushes of wave w are done
     cluster_wait_acquire();
@@ -316,7 +291,7 @@ static bool moe_carve(const Layout &L, int T, int c, int S, MoePlan &m) {
   m.grid = m.nb * c;
   const int xb = m.ng_max * kMoeN * 256, recv = 2 * c * T * 512;
   const int fixed = xb + kMoeRotBytes + recv + kMoeTabBytes + kMoeBarBytes + 128;
-  const int nst = ring_stages(kMoeSmemLimit - fixed, L.rec_bytes, kMoeMaxStages, 1, 4, false);
+  const int nst = ring_stages(kMoeSmemLimit - fixed, L.rec_bytes, kMoeMaxStages, 2, 4, false);   // even: segment_rounds
   if (!nst) return false;
   m.nstages = nst;
   m.xb_off = (nst * L.rec_bytes + 127) / 128 * 128;

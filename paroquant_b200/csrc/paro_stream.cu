@@ -366,10 +366,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
 
   if (warp == kProdWarp) {
     // every worker warp consumes every ring stage and contributes to every segment accumulator
-    if (lane < NS) {
-      mbar_init(bar_wfull + 8 * lane, 1);
-      mbar_init(bar_wempty + 8 * lane, kWorkers);
-    }
+    ring_init(bar_wfull, bar_wempty, NS, kWorkers, lane);
     if (lane < kStmDBufs) {
       mbar_init(bar_dfull + 8 * lane, kWorkers);
       mbar_init(bar_dfree + 8 * lane, 4);
@@ -383,7 +380,8 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
     // ================= producer: ONE bulk copy per round; nothing here depends on activations, so it runs ahead across
     // step boundaries.  The whole warp runs the loop, an elected lane issues.
     const uint64_t pol = policy_evict_first();
-    int st = 0, it = 0, lag_st = 0, lag_it = 0;   // lag_*: stage / wrap of copy number (issued - inflight)
+    RingProducer prod = {bar_wfull, bar_wempty, smem0, static_cast<uint32_t>(p.stage_bytes), NS, 0, 0};
+    int lag_st = 0, lag_it = 0;   // stage / wrap of copy number (issued - inflight)
     uint32_t issued = 0;
 #pragma unroll 1
     for (int i = 0; i < nsteps; ++i) {
@@ -401,15 +399,9 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
         int gi = ra - jb * g.ng;
 #pragma unroll 1
         for (int r = ra; r < rb; ++r, ++gi) {
-          if (it > 0) mbar_wait(bar_wempty + 8 * st, (it - 1) & 1);
           // at most `inflight` records outstanding per SM (the stage of copy n - inflight has not been reused yet)
           if (issued >= static_cast<uint32_t>(p.inflight)) mbar_wait(bar_wfull + 8 * lag_st, lag_it & 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(bar_wfull + 8 * st, rec_bytes);
-            bulk_g2s(smem0 + st * p.stage_bytes, rec_part + (static_cast<size_t>(jb) * S.groups + gi) * rec_bytes, rec_bytes, bar_wfull + 8 * st, pol);
-          }
-          __syncwarp();
-          if (++st == NS) { st = 0; ++it; }
+          prod.issue([=, &S] { return rec_part + (static_cast<size_t>(jb) * S.groups + gi) * rec_bytes; }, rec_bytes, pol, [] {});
           if (++issued > static_cast<uint32_t>(p.inflight)) {
             if (++lag_st == NS) { lag_st = 0; ++lag_it; }
           }

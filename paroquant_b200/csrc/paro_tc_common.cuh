@@ -1,5 +1,6 @@
 // Device helpers shared by the tensor-core kernels (paro_decode.cu, paro_stream.cu, paro_moe.cu, paro_gemm.cu):
-// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T A-fragment dequant,
+// mma.sync / wgmma wrappers and operand fragments, cluster + DSMEM primitives, the INT4 -> T A-fragment dequant, the small-M
+// kernels' weight ring (set-up, producer step, round loop),
 // the in-warp pairwise rotation (rounding points of /root/reference/paroquant/kernels/cuda/rotation.cuh:91-173) and the
 // small-M kernels' rotation prologue built from it (rotation_tasks).
 #pragma once
@@ -239,7 +240,37 @@ __device__ __forceinline__ void mma_rounds(uint32_t rec, uint32_t rec_stride, ui
   }
 }
 
-// ------------------------------------------------------------------ round loop of the small-M kernels (decode)
+// ------------------------------------------------------------------ weight ring of the small-M kernels (decode, stream, MoE)
+// `nstages` stages of one record each, every stage with a full barrier (the producer's expect_tx, then the bulk copy's bytes)
+// and an empty barrier (one arrival per consumer warp), 8 bytes apart from `full` / `empty`.  One barrier pair per lane of the
+// calling warp; the caller initialises its own other barriers and then fences them all (fence_mbar_init).
+__device__ __forceinline__ void ring_init(uint32_t full, uint32_t empty, int nstages, int consumers, int lane) {
+  if (lane < nstages) {
+    mbar_init(full + 8 * lane, 1);
+    mbar_init(empty + 8 * lane, consumers);
+  }
+}
+
+// The producer warp's place in the ring: stage `st` of wrap `it`.  The whole warp calls issue(), which waits until the stage's
+// previous record was consumed, then one elected lane arms the full barrier, starts the bulk copy of `bytes` from src() into
+// the stage and runs on_issue().  src is a hook so that the address arithmetic stays behind the wait, where the producer loops
+// had it (computed ahead, it reorders decode_kernel's instructions).
+struct RingProducer {
+  uint32_t full, empty, stage0, stride;   // barrier bases, stage 0's address, stage stride
+  int nstages, st, it;
+  template <typename Src, typename OnIssue>
+  __device__ __forceinline__ void issue(Src src, uint32_t bytes, uint64_t policy, OnIssue on_issue) {
+    if (it > 0) mbar_wait(empty + 8 * st, (it - 1) & 1);
+    if (elect_one()) {
+      mbar_arrive_expect_tx(full + 8 * st, bytes);
+      bulk_g2s(stage0 + st * stride, src(), bytes, full + 8 * st, policy);
+      on_issue();
+    }
+    __syncwarp();
+    if (++st == nstages) { st = 0; ++it; }
+  }
+};
+
 // A worker warp's place in the weight ring: `fb` = full barrier of the next stage to take, its empty barrier sits `empty_off`
 // above; stage records are rec_stride apart, the record of a stage is fb * rec_per_bar + rec_at_bar0.
 struct RingCursor {
@@ -259,8 +290,9 @@ struct RingCursor {
 
 // The round loop of a worker warp over `nseg` segments (runs of consecutive records that go into one accumulator):
 // seg_begin(k, bx, len) gives segment k's first B row and record count, seg_end(k, acc) hands its accumulator on.  Records
-// are taken in pairs from an even stage (the ring depth is even: a pair never wraps); a segment that starts at an odd stage
-// takes its first record alone, an odd remainder its last.  The loop counts the records left in the segment.
+// are taken in pairs from an even stage; a segment that starts at an odd stage takes its first record alone, an odd remainder
+// its last.  The loop counts the records left in the segment.
+// The ring depth must be even, so that a pair never wraps: every caller's depth rule (ring_stages) rounds to a multiple of 2.
 // seen(n) / done(n): tracing hooks after n records' full barriers were seen / their MMAs issued.
 template <typename T, int NTT, int NR, typename SegBegin, typename SegEnd, typename Seen, typename Done>
 __device__ __forceinline__ void segment_rounds(RingCursor &rg, const RoundLane &lo, int nseg, SegBegin seg_begin, SegEnd seg_end, Seen seen,
@@ -303,6 +335,22 @@ __device__ __forceinline__ void segment_rounds(RingCursor &rg, const RoundLane &
       seg_end(k, acc);
       ++k;
     }
+  }
+}
+
+// The two k-half warps of a tile add their accumulators in a fixed order: the k-half-1 warp stores its 8 values per lane at
+// xc, xc + 128, ..., both pass the tile's pair barrier `bar`, and the k-half-0 warp adds them to its own and runs sum().
+template <typename Sum>
+__device__ __forceinline__ void khalf_meet(float (&acc)[2][4], uint32_t xc, int kh, int bar, Sum sum) {
+  if (kh == 1) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) sts_f32(xc + i * 128, acc[i >> 2][i & 3]);
+  }
+  named_bar_sync(bar, 64);
+  if (kh == 0) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i >> 2][i & 3] += lds_f32(xc + i * 128);
+    sum();
   }
 }
 

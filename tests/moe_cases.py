@@ -8,13 +8,13 @@ Plans at 132 SMs (cluster size c, K slices S; waves at U_max = min(E, T * k)):
   H, I, E          T, k   dtype, group, krot   gate_up                                  down
   256, 8192, 8     4, 1   bf16, 128, 8         c = 1, 4 waves                           c = 8, S = 2, 32 groups per item on 4 stages
   1024, 4096, 64   9, 1   bf16, 128, 8         c = 2, S = 2, 9 waves                    c = 8, S = 7 (an expert's slices cross a wave), 8 waves
-  4096, 1536, 64   9, 1   fp16, 64, 3          c = 4, S = 2, 16 groups on 11 stages     c = 4, S = 3 (crosses waves), 7 waves
+  4096, 1536, 64   9, 1   fp16, 64, 3          c = 4, S = 2, 16 groups on 10 stages     c = 4, S = 3 (crosses waves), 7 waves
   4096, 14336, 8   1, 2   bf16, 128, 8         c = 4, S = 2                             c = 4, S = 4, 28 groups per item on 10 stages
   4096, 14336, 8   16, 2  fp16, 64, 5          c = 4, S = 2, 16 groups on 8 stages      c = 4, S = 7 (crosses waves), 14 waves, 16 groups on 8 stages
   4096, 128, 64    9, 1   bf16, 128, 8         c = 8, S = 7 of 32 groups (uneven)       c = 4, S = 1, 3 waves (the last partial)
   256, 128, 1      1, 1   bf16, 128, 8         c = 2, S = 2                             c = 1
   256, 128, 8      1, 2   fp16, 128, 8         c = 4, S = 2                             c = 2, S = 1
-  2048, 768, 128   16, 8  bf16, 128, 8         c = 8, S = 2, 32 waves, 8 groups on 4    c = 8, 16 waves, 6 groups on 5 stages
+  2048, 768, 128   16, 8  bf16, 128, 8         c = 8, S = 2, 32 waves, 8 groups on 4    c = 8, 16 waves, 6 groups on 4 stages
   256, 384, 32     8, 16  bf16, 128, 8         c = 8, 4 waves                           c = 8, 4 waves
 
 (the two Mixtral-shaped rows are Mixtral-8x7B's expert shapes, the 2048 / 768 / 128 row Qwen3-30B-A3B's)
