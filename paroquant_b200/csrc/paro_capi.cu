@@ -87,6 +87,13 @@ int ring_stages(int room, int stage_bytes, int max_stages, int multiple, int min
 
 static bool valid_dtype(int d) { return d == PARO_F32 || d == PARO_F16 || d == PARO_BF16; }
 static bool aligned(const void *p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+// the layout of a linear's shape; on a null or unsupported shape false, with the error "<what>: <reason>"
+static bool layout_of(const paro_linear_shape *shape, const char *what, Layout &L) {
+  const char *why = "null shape";
+  if (shape && make_layout(*shape, L, &why)) return true;
+  set_error("%s: %s", what, why);
+  return false;
+}
 
 }  // namespace paro
 
@@ -138,8 +145,7 @@ int paro_rotate_backward(const void *y, const void *grad_out, const void *x, con
 
 size_t paro_packed_bytes(const paro_linear_shape *shape) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("packed_bytes: %s", shape ? why : "null shape"); return 0; }
+  if (!layout_of(shape, "packed_bytes", L)) return 0;
   return L.total_bytes;
 }
 
@@ -148,8 +154,7 @@ int paro_prepack(const paro_linear_shape *shape, const int32_t *qweight, const i
                  const void *channel_scales, int32_t cs_dtype, void *packed, paro_stream_t stream) {
   g_launches = 0;
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("prepack: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "prepack", L)) return PARO_EINVAL;
   if (!qweight || !qzeros || !scales || !pairs || !theta || !channel_scales || !packed) { set_error("prepack: null pointer argument"); return PARO_EINVAL; }
   if (!valid_dtype(scales_dtype) || !valid_dtype(theta_dtype) || !valid_dtype(cs_dtype)) { set_error("prepack: bad parameter dtype"); return PARO_EINVAL; }
   if (!aligned(packed, 128)) { set_error("prepack: packed buffer must be 128-byte aligned"); return PARO_EINVAL; }
@@ -159,8 +164,7 @@ int paro_prepack(const paro_linear_shape *shape, const int32_t *qweight, const i
 
 size_t paro_workspace_bytes(const paro_linear_shape *shape, int64_t max_m) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("workspace_bytes: %s", shape ? why : "null shape"); return 0; }
+  if (!layout_of(shape, "workspace_bytes", L)) return 0;
   // head: sync words + block counters of the small-M kernel (zero between calls); behind them scratch: the partial slots
   // of the small-M kernel or the rotated activations of the M > 16 path
   size_t b = stream_workspace_bytes(L, max_m);
@@ -179,8 +183,7 @@ int paro_linear_forward(const paro_linear_shape *shape, const void *packed, cons
                         void *y, void *workspace, size_t workspace_bytes, paro_stream_t stream) {
   g_launches = 0;
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("linear_forward: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "linear_forward", L)) return PARO_EINVAL;
   if (M < 0) { set_error("linear_forward: negative row count"); return PARO_EINVAL; }
   if (M == 0) return PARO_OK;
   if (!packed || !x || !y || !workspace) { set_error("linear_forward: null pointer argument"); return PARO_EINVAL; }
@@ -189,6 +192,12 @@ int paro_linear_forward(const paro_linear_shape *shape, const void *packed, cons
     return PARO_EINVAL;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // outside the cluster kernel a single linear runs as a one-step chain: the chain kernel up to 16 rows, the prefill chain above
+  HostStep h = {};
+  h.shape = shape;
+  h.L = L;
+  h.packed = packed; h.bias = bias; h.x = x; h.y = y;
+  h.x_op = PARO_XOP_NONE; h.epi_op = PARO_EPI_STORE;
   if (M <= knobs().small_m_max) {
     // A single linear: the cluster kernel (paro_decode.cu: K slices reduced through distributed shared memory) has the shorter
     // tail -- measured 7.4 / 9.9 / 22.0 / 15.6 us on the Llama-3-8B shapes at M = 1 against 11.1 / 12.3 / 24.3 / 16.2 us for
@@ -200,18 +209,17 @@ int paro_linear_forward(const paro_linear_shape *shape, const void *packed, cons
                                     workspace_bytes > head ? workspace_bytes - head : 0, st);
       if (rc != PARO_EUNSUPPORTED) return rc;
     }
-    return stream_linear_forward(*shape, L, packed, x, M, bias, y, workspace, workspace_bytes, st);
+    return stream_forward(&h, 1, M, workspace, workspace_bytes, st);
   }
   const size_t head = stream_sync_bytes(L);   // never touched by the large-M path
   if (workspace_bytes < head) { set_error("workspace too small: have %zu, need %zu", workspace_bytes, head); return PARO_EWORKSPACE; }
-  return gemm_forward(*shape, L, packed, x, M, bias, y, static_cast<uint8_t *>(workspace) + head, workspace_bytes - head, st);
+  return prefill_chain_forward(&h, 1, M, static_cast<uint8_t *>(workspace) + head, workspace_bytes - head, st);
 }
 
 int paro_unpack_dense(const paro_linear_shape *shape, const void *packed, void *W_out, paro_stream_t stream) {
   g_launches = 0;
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("unpack_dense: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "unpack_dense", L)) return PARO_EINVAL;
   if (!packed || !W_out) { set_error("unpack_dense: null pointer argument"); return PARO_EINVAL; }
   return unpack_dense_launch(*shape, L, packed, W_out, static_cast<cudaStream_t>(stream));
 }
@@ -228,16 +236,14 @@ int paro_debug_silu_mul(int32_t dtype, const void *gate_up, void *act, int64_t M
 int paro_debug_decode_plan(const paro_linear_shape *shape, int64_t M, int32_t sets, int32_t sms, const int32_t *resident_clusters,
                             int32_t *out) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_decode_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "debug_decode_plan", L)) return PARO_EINVAL;
   if (!resident_clusters || !out || sms < 1) { set_error("debug_decode_plan: bad arguments"); return PARO_EINVAL; }
   return decode_debug_plan(L, M, sets, sms, resident_clusters, out);
 }
 
 int paro_debug_gemm_plan(const paro_linear_shape *shape, int64_t M, int32_t sms, int32_t *out) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_gemm_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "debug_gemm_plan", L)) return PARO_EINVAL;
   if (!out) { set_error("debug_gemm_plan: bad arguments"); return PARO_EINVAL; }
   return gemm_debug_plan(L, M, sms, out);
 }
@@ -357,16 +363,14 @@ int paro_prefill_chain_forward(const paro_chain_step *steps, int32_t n_steps, in
 
 size_t paro_tp_slot_bytes(const paro_linear_shape *shape, int64_t M, int32_t world) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("tp_slot_bytes: %s", shape ? why : "null shape"); return 0; }
+  if (!layout_of(shape, "tp_slot_bytes", L)) return 0;
   if (M < 1 || M > 16 || world < 1 || world > PARO_TP_MAX_RANKS) { set_error("tp_slot_bytes: 1 <= M <= 16, 1 <= world <= %d", PARO_TP_MAX_RANKS); return 0; }
   return static_cast<size_t>(2) * L.blocks_total * world * M * 128 * 8;
 }
 
 int paro_debug_stream_plan(const paro_linear_shape *shape, int64_t M, int32_t sets, int32_t ctas, int32_t *out) {
   Layout L;
-  const char *why = "";
-  if (!shape || !make_layout(*shape, L, &why)) { set_error("debug_stream_plan: %s", shape ? why : "null shape"); return PARO_EINVAL; }
+  if (!layout_of(shape, "debug_stream_plan", L)) return PARO_EINVAL;
   if (!out) { set_error("debug_stream_plan: bad arguments"); return PARO_EINVAL; }
   return stream_debug_plan(L, M, sets, ctas, out);
 }

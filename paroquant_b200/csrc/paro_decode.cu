@@ -37,7 +37,7 @@ constexpr int kDecN = 16;            // B operand rows per group: token rows, ze
 constexpr int kDecSmemLimit = 227 * 1024;
 constexpr int kDecBarBytes = 16 * kDecMaxStages + 256;   // ring barriers + the x-load barrier
 constexpr int kDecXchgBytes = 2 * 8 * 8 * 128;           // k-half partials: [2][8 tiles][8 values][32 lanes] fp32 (in the rotation tiles)
-// one record per ring stage: 8576 bytes (group_size 128) or 8960 (group_size 64), both multiples of 64 -> DecParams::rec_bytes
+// one record per ring stage: 8576 bytes (group_size 128) or 8960 (group_size 64), both multiples of 64 -> Layout::rec_bytes
 
 constexpr int kDecTraceSlots = 12;
 constexpr int kDecTraceCtas = 200;       // rows 200.. of the trace double as a per-round log of CTA 0 (issued / full / consumed)
@@ -54,26 +54,21 @@ struct DecParams {
   const void *x;
   void *y;
   const void *bias;
-  int M, K, N;
-  int n_parts, groups, krot;
+  Layout L;                       // the packed linear (paro_layout.h); a record is one ring stage
+  int M;
   int c, c_shift;                 // cluster size (K slices of this launch), log2
   int nstages, rot_bytes, rot_warps, trace;   // rot_warps: worker warps that take rotation tasks (each owns one rot_bytes tile)
-  int rec_bytes, q2;              // record (= ring stage) size; q2: group_size 64, two scale / zero sets per record (paro_layout.h)
   int pre_rotated;                // x is the pre-pass's output: [n_parts][M][K], already scaled and rotated (no stages here)
   long long x_part_stride;        // elements between partitions of a pre-rotated x (0 otherwise)
   int xb_off, rot_off, recv_off, bar_off;   // shared-memory carve-up (bytes)
-  int part_col_begin[PARO_MAX_PARTS + 1];
-  int part_block_begin[PARO_MAX_PARTS + 1];
   int part_range_begin[PARO_MAX_PARTS + 1];
-  int meta_group_bytes;
-  long long meta_off, rec_off;
 };
 
 template <typename T>
 __device__ __forceinline__ void dec_store(const DecParams &p, float v, int m, int n) {
   T t = Traits<T>::from_float(v);
   if (p.bias) t = Traits<T>::from_float(Traits<T>::to_float(t) + Traits<T>::to_float(static_cast<const T *>(p.bias)[n]));  // plugin.py:309-310
-  static_cast<T *>(p.y)[static_cast<int64_t>(m) * p.N + n] = t;
+  static_cast<T *>(p.y)[static_cast<int64_t>(m) * p.L.N + n] = t;
 }
 
 template <typename T>
@@ -98,27 +93,27 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
   while (range >= p.part_range_begin[part + 1]) ++part;
   const int jl = range - p.part_range_begin[part];
   const int cp = p.part_range_begin[part + 1] - p.part_range_begin[part];
-  const int cbp = p.part_block_begin[part + 1] - p.part_block_begin[part];
+  const int cbp = p.L.part_block_begin[part + 1] - p.L.part_block_begin[part];
   const int cb_begin = static_cast<int>(static_cast<unsigned>(jl) * static_cast<unsigned>(cbp) / static_cast<unsigned>(cp));
   const int cb_end = static_cast<int>(static_cast<unsigned>(jl + 1) * static_cast<unsigned>(cbp) / static_cast<unsigned>(cp));
   const int nj = cb_end - cb_begin;
-  const int g_begin = static_cast<int>(static_cast<unsigned>(slice) * static_cast<unsigned>(p.groups) >> p.c_shift);
-  const int g_end = static_cast<int>(static_cast<unsigned>(slice + 1) * static_cast<unsigned>(p.groups) >> p.c_shift);
+  const int g_begin = static_cast<int>(static_cast<unsigned>(slice) * static_cast<unsigned>(p.L.groups) >> p.c_shift);
+  const int g_end = static_cast<int>(static_cast<unsigned>(slice + 1) * static_cast<unsigned>(p.L.groups) >> p.c_shift);
   const int ng = g_end - g_begin;
   const int nrounds = nj * ng;
   // first output column of my first block, and the end of my partition (a last partial block is masked at the stores)
-  const int n_first = p.part_col_begin[part] + cb_begin * kBlockN, n_end = p.part_col_begin[part + 1];
+  const int n_first = p.L.part_col_begin[part] + cb_begin * kBlockN, n_end = p.L.part_col_begin[part + 1];
   // record of (block j, group gi) of mine: rec0 + (j * groups + gi) * rec_bytes
-  const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
-  const uint8_t *rec0 = p.packed + p.rec_off + (static_cast<size_t>(p.part_block_begin[part] + cb_begin) * p.groups + g_begin) * rec_bytes;
+  const uint32_t rec_bytes = static_cast<uint32_t>(p.L.rec_bytes);
+  const uint8_t *rec0 = p.packed + p.L.rec_off + (static_cast<size_t>(p.L.part_block_begin[part] + cb_begin) * p.L.groups + g_begin) * rec_bytes;
 
   // A rotation task = (group of the slice, block of up to 4 token rows); worker warp w takes tasks w, w + rot_warps, ...  (M = 16:
   // four tasks per group, so all warps share the rotation instead of 16-row tiles on a few)
   RotMeta rm;
   const int nq = p.M > 4 ? (p.M + 3) >> 2 : 1, ntasks = ng * nq;
-  const int mi0 = part * p.groups + g_begin;   // metadata block of the slice's first group
+  const int mi0 = part * p.L.groups + g_begin;   // metadata block of the slice's first group
   if (!p.pre_rotated && warp < kWorkers && warp < ntasks && warp < p.rot_warps)
-    fetch_meta(p.packed + p.meta_off + static_cast<size_t>(mi0 + warp / nq) * p.meta_group_bytes, p.krot, lane, rm);   // flies during the barrier initialisation
+    fetch_meta(p.packed + p.L.meta_off + static_cast<size_t>(mi0 + warp / nq) * p.L.meta_group_bytes, p.L.krot, lane, rm);   // flies during the barrier initialisation
 
   if (warp == kWorkers) {
     ring_init(bar_wfull, bar_wempty, NS, kWorkers, lane);   // every worker warp consumes every ring stage
@@ -140,7 +135,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
 #pragma unroll 1
     for (int r = 0; r < nrounds; ++r) {
       // (hooks that capture the loop counters by reference change the instructions nvcc makes of this loop)
-      prod.issue([=, &p] { return rec0 + (static_cast<size_t>(j) * p.groups + gi) * rec_bytes; }, rec_bytes, pol, [=, &p] {
+      prod.issue([=, &p] { return rec0 + (static_cast<size_t>(j) * p.L.groups + gi) * rec_bytes; }, rec_bytes, pol, [=, &p] {
         if (p.trace && blockIdx.x == 0 && r < 100) g_dec_trace[kDecTraceCtas * kDecTraceSlots + 3 * r] = clock64() - t_entry;
       });
       if (++gi == ng) { gi = 0; ++j; }
@@ -175,7 +170,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
       if (wi < ntasks && wi < p.rot_warps) {
         const uint32_t rot = smem0 + p.rot_off + wi * p.rot_bytes;
         const int M = p.M, rw = p.rot_warps;
-        const uint8_t *meta = p.packed + p.meta_off;
+        const uint8_t *meta = p.packed + p.L.meta_off;
         auto stage_x = [&](auto rows, int gi, int m0, uint2 csw) {
           constexpr int ROWS = decltype(rows)::value;
           const T *xg = static_cast<const T *>(p.x) + (g_begin + gi) * kGroup + 4 * lane;
@@ -183,14 +178,14 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
 #pragma unroll
           for (int m = 0; m < ROWS; ++m) {
             raw[m] = make_uint2(0u, 0u);
-            if (m0 + m < M) raw[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * p.K));
+            if (m0 + m < M) raw[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * p.L.K));
           }
           scale_and_stage<T, ROWS>(rot, lane, raw, csw);
           if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 0] = clock64() - t_entry;
         };
-        if (M == 1) rotation_tasks<T, 1, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
-        else if (M == 2) rotation_tasks<T, 2, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
-        else rotation_tasks<T, 4, true>(rm, meta, p.meta_group_bytes, p.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        if (M == 1) rotation_tasks<T, 1, true>(rm, meta, p.L.meta_group_bytes, p.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        else if (M == 2) rotation_tasks<T, 2, true>(rm, meta, p.L.meta_group_bytes, p.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
+        else rotation_tasks<T, 4, true>(rm, meta, p.L.meta_group_bytes, p.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, kDecN, stage_x);
         if (p.trace && threadIdx.x == 0 && blockIdx.x < kDecTraceCtas) g_dec_trace[blockIdx.x * kDecTraceSlots + 9] = clock64() - t_entry;
       }
       named_bar_sync(2, 32 * kWorkers);   // B operand complete
@@ -199,7 +194,7 @@ __global__ void __launch_bounds__(32 * (kDecWorkers + 1), 1) decode_kernel(const
 
     const int M = p.M;
     const int g = lane >> 2, t = lane & 3;
-    const RoundLane lo = round_lane<kDecN>(p.q2 != 0, tile, kh, lane);
+    const RoundLane lo = round_lane<kDecN>(p.L.qhalves == 2, tile, kh, lane);
     // The round loop (segment_rounds: one segment = one 128-column block), specialised on the token tiles (NTT) and on
     // tracing, so that neither is a per-round branch.
     using One = std::integral_constant<int, 1>;
@@ -425,14 +420,14 @@ static bool dec_cached_plan(const Layout &L, int M, int sms, DecCached &out) {
 }
 
 template <typename T>
-static int launch_decode(DecParams &p, const Layout &L, const DecCached &c, cudaStream_t stream) {
+static int launch_decode(DecParams &p, const DecCached &c, cudaStream_t stream) {
   auto kern = decode_kernel<T>;
   const Knobs &kn = knobs();
   const DecPlan &best = c.plan;
   const DecSmem &best_s = c.smem;
   if (kn.verbose)
     fprintf(stderr, "[paro decode] K=%d N=%d M=%d: cluster %d x %d ranges (grid %d), blocks/CTA <= %d, groups/CTA <= %d, %d stages, smem %d\n",
-            L.K, L.N, p.M, best.c, best.ranges, best.grid, best.nj_max, best.ng_max, best_s.nstages, best_s.total);
+            p.L.K, p.L.N, p.M, best.c, best.ranges, best.grid, best.nj_max, best.ng_max, best_s.nstages, best_s.total);
 
   PARO_CUDA_OK(smem_opt_in(kern, kDecSmemLimit));
   cudaLaunchConfig_t cfg;
@@ -480,7 +475,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   const size_t part_bytes = static_cast<size_t>(kDecN) * L.K * 2;   // 16 rows (zero padded) x K of T, B-operand order
   const bool prerot = decode_wants_prerot(L, M) && scratch && scratch_bytes >= L.n_parts * part_bytes;
   if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_small_kernel)
-    const int rc = rotate_small_launch(L, packed, x, scratch, M, kDecN, kDecN, stream);
+    const int rc = rotate_chain_launch(L, packed, PARO_XOP_NONE, x, nullptr, nullptr, 0, 0.f, scratch, M, kDecN, kDecN, stream);
     if (rc) return rc;
   }
   DecParams p = {};
@@ -488,19 +483,11 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   p.x = prerot ? scratch : x; p.y = y; p.bias = bias;
   p.pre_rotated = prerot ? 1 : 0;
   p.x_part_stride = prerot ? static_cast<long long>(kDecN) * L.K : 0;
-  p.M = static_cast<int>(M); p.K = L.K; p.N = L.N;
-  p.n_parts = L.n_parts; p.groups = L.groups; p.krot = L.krot;
-  p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2;
+  p.L = L;
+  p.M = static_cast<int>(M);
   p.rot_bytes = dec_rot_bytes(M);
   p.trace = knobs().trace;
-  for (int i = 0; i <= PARO_MAX_PARTS; ++i) {
-    p.part_col_begin[i] = L.part_col_begin[i];
-    p.part_block_begin[i] = L.part_block_begin[i];
-  }
-  p.meta_group_bytes = L.meta_group_bytes;
-  p.meta_off = static_cast<long long>(L.meta_off);
-  p.rec_off = static_cast<long long>(L.rec_off);
-  return s.dtype == PARO_BF16 ? launch_decode<__nv_bfloat16>(p, L, plan, stream) : launch_decode<__half>(p, L, plan, stream);
+  return s.dtype == PARO_BF16 ? launch_decode<__nv_bfloat16>(p, plan, stream) : launch_decode<__half>(p, plan, stream);
 }
 
 }  // namespace paro

@@ -35,12 +35,9 @@ struct GemmParams {
   const uint8_t *xr;       // [n_parts][token blocks][K/16 steps][2][NT/8][8][8] elements
   void *y;
   const void *bias;
-  int M, K, N, NT, n_blocks, tok_blocks;
-  int n_parts, groups;
-  int rec_bytes, q2;       // record size; q2: group_size 64, two scale / zero sets per record (paro_layout.h)
-  int part_col_begin[PARO_MAX_PARTS + 1];
-  int part_block_begin[PARO_MAX_PARTS + 1];
-  long long rec_off, xr_part_stride;
+  Layout L;                // the packed linear (paro_layout.h)
+  int M, NT, tok_blocks;
+  long long xr_part_stride;
 };
 
 // Tile source of a linear: token block tb is rows tb * NT .. tb * NT + NT - 1 of x and y, the weights are p.packed.
@@ -56,7 +53,7 @@ struct ResidualTiles {
   static constexpr bool kGrouped = false, kResidual = true;
   const void *res_in;
   void *res_out;
-  float *stats;   // [n_blocks][M] or NULL
+  float *stats;   // [blocks_total][M] or NULL
 };
 // Tile source of a MoE block's grouped GEMM: tile slot tb is positions tb * NT .. of the routing table, all of one expert
 // (paro_moe_grouped.cu writes the table on the device).  Slots from *live_tiles on are empty and exit at once.
@@ -106,7 +103,7 @@ __device__ __forceinline__ void residual_epilogue(const GemmParams &p, const Res
         if (m < p.M) {
           T v = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
           if (has_bias) v = Traits<T>::from_float(Traits<T>::to_float(v) + bias_f);
-          const int64_t o = m * p.N + nn;
+          const int64_t o = m * p.L.N + nn;
           if (yout) yout[o] = v;
           const T h = Traits<T>::from_float(Traits<T>::to_float(v) + Traits<T>::to_float(rin[o]));
           rout[o] = h;
@@ -146,11 +143,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
   const uint32_t bars = b_ring + kBStages * b_stage_bytes;
   const uint32_t bar_wfull = bars, bar_wempty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 160;
 
-  const int block = blockIdx.x % p.n_blocks, tb = blockIdx.x / p.n_blocks;   // 128-column block (over all partitions), token block
+  const int block = blockIdx.x % p.L.blocks_total, tb = blockIdx.x / p.L.blocks_total;   // 128-column block (over all partitions), token block
   int part = 0;
-  while (block >= p.part_block_begin[part + 1]) ++part;
-  const int n0 = p.part_col_begin[part] + (block - p.part_block_begin[part]) * kBlockN, n_end = p.part_col_begin[part + 1];
-  const int rounds = p.groups;
+  while (block >= p.L.part_block_begin[part + 1]) ++part;
+  const int n0 = p.L.part_col_begin[part] + (block - p.L.part_block_begin[part]) * kBlockN, n_end = p.L.part_col_begin[part + 1];
+  const int rounds = p.L.groups;
   const uint8_t *packed = p.packed;
   if constexpr (Tiles::kGrouped) {
     pdl_wait();   // the routing table (written two launches back) names the tile's expert
@@ -169,8 +166,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     // ================= weight producer: independent of the pre-pass; every 128-column block is re-read by
     // all token blocks, so the records stay under the normal L2 policy (no evict-first here)
     if (lane == 0) {
-      const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
-      const uint8_t *rec = packed + p.rec_off + static_cast<size_t>(block) * p.groups * rec_bytes;
+      const uint32_t rec_bytes = static_cast<uint32_t>(p.L.rec_bytes);
+      const uint8_t *rec = packed + p.L.rec_off + static_cast<size_t>(block) * p.L.groups * rec_bytes;
       for (int r = 0; r < rounds; ++r) {
         const int ws = r % kWStages, wit = r / kWStages;
         if (wit > 0) mbar_wait(bar_wempty + 8 * ws, (wit - 1) & 1);
@@ -184,7 +181,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     // ================= x_rot producer: one contiguous NT x 64 operand tile per stage
     if (lane == 0) {
       const uint8_t *xr_tile = p.xr + static_cast<size_t>(part) * p.xr_part_stride +
-                               static_cast<size_t>(tb) * (p.K / 64) * b_stage_bytes;
+                               static_cast<size_t>(tb) * (p.L.K / 64) * b_stage_bytes;
       pdl_wait();   // x_rot is written by the pre-pass kernel
       for (int bi = 0; bi < 2 * rounds; ++bi) {
         const int bs = bi % kBStages, bit = bi / kBStages;
@@ -201,7 +198,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
     const int wg = (warp >> 2) - 1, w = warp & 3;
     const int g = lane >> 2, t = lane & 3;
     const int tile = 4 * wg + w, r = 16 * tile + g;   // my 16-row tile, rows r and r + 8 inside the block
-    const bool q2 = p.q2 != 0;
+    const bool q2 = p.L.qhalves == 2;
     const uint32_t zero_off = q2 ? block_zero_off(2) : block_zero_off(1);
     const uint64_t desc_hi = smem_desc_kmajor(0, NT * 16, 128);
     float acc[NT / 2];
@@ -277,11 +274,11 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wg_gemm_kernel(const GemmPara
           const int64_t m = static_cast<int64_t>(tb) * NT + 8 * j + 2 * t + e;
           if constexpr (Tiles::kGrouped) {
             const int row = tiles.rows[m];
-            if (row >= 0) yout[static_cast<int64_t>(row) * p.N + n] = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
+            if (row >= 0) yout[static_cast<int64_t>(row) * p.L.N + n] = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
           } else if (m < p.M) {
             T v = Traits<T>::from_float(acc[4 * j + 2 * hi + e]);
             if (has_bias) v = Traits<T>::from_float(Traits<T>::to_float(v) + bias_f);
-            yout[m * p.N + n] = v;
+            yout[m * p.L.N + n] = v;
           }
         }
       }
@@ -333,7 +330,7 @@ static int launch_gemm(const GemmParams &p, const Tiles &tiles, cudaStream_t str
   PARO_CUDA_OK(smem_opt_in(kern, static_cast<int>(smem)));
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[2];
-  launch_config(cfg, attr, p.n_blocks * p.tok_blocks, kGemmThreads, smem, stream, 0, true);   // PDL: prologue + first weight stages overlap the pre-pass
+  launch_config(cfg, attr, p.L.blocks_total * p.tok_blocks, kGemmThreads, smem, stream, 0, true);   // PDL: prologue + first weight stages overlap the pre-pass
   PARO_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p, tiles));
   note_launches(1);
   return PARO_OK;
@@ -346,18 +343,6 @@ static int launch_gemm_nt(const GemmParams &p, cudaStream_t stream, const Tiles 
   return launch_gemm<T, 32>(p, tiles, stream);
 }
 
-static void fill_weights(GemmParams &p, const Layout &L) {
-  p.K = L.K; p.N = L.N;
-  p.n_blocks = L.blocks_total;
-  p.n_parts = L.n_parts; p.groups = L.groups;
-  p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2;
-  for (int i = 0; i <= PARO_MAX_PARTS; ++i) {
-    p.part_col_begin[i] = L.part_col_begin[i];
-    p.part_block_begin[i] = L.part_block_begin[i];
-  }
-  p.rec_off = static_cast<long long>(L.rec_off);
-}
-
 // a linear's GEMM over M rows in tiles of NT, x_rot (m_pad rows per partition) at xr
 static GemmParams dense_params(const Layout &L, const void *packed, const void *xr, void *y, const void *bias, int64_t M, int NT, int64_t m_pad) {
   GemmParams p;
@@ -365,30 +350,11 @@ static GemmParams dense_params(const Layout &L, const void *packed, const void *
   p.xr = static_cast<const uint8_t *>(xr);
   p.y = y;
   p.bias = bias;
-  fill_weights(p, L);
+  p.L = L;
   p.M = static_cast<int>(M); p.NT = NT;
   p.tok_blocks = static_cast<int>(m_pad / NT);
   p.xr_part_stride = static_cast<long long>(m_pad) * L.K * 2;
   return p;
-}
-
-int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
-                 const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (workspace_bytes < gemm_workspace_bytes(L, M)) {
-    set_error("workspace too small: have %zu, need %zu", workspace_bytes, gemm_workspace_bytes(L, M));
-    return PARO_EWORKSPACE;
-  }
-  const int NT = pick_nt(M, L, planning_sms());
-  const int64_t m_pad = (M + NT - 1) / NT * NT;
-  // ---- pre-pass: ONE launch rotates x for every partition, output in B-operand tile order (paro_rotate.cu: rotate_small_kernel
-  // fetches all stage parameters up front; the per-partition rotate_kernel launches it replaces cost 3 x ~7 us at 256 tokens)
-  {
-    const int rc = rotate_small_launch(L, packed, x, workspace, M, m_pad, NT, stream);
-    if (rc) return rc;
-  }
-  const GemmParams p = dense_params(L, packed, workspace, y, bias, M, NT, m_pad);
-  if (s.dtype == PARO_BF16) return launch_gemm_nt<__nv_bfloat16>(p, stream);
-  return launch_gemm_nt<__half>(p, stream);
 }
 
 // ------------------------------------------------------------------ prefill chain (paro_prefill_chain_forward)
@@ -427,7 +393,8 @@ static PrefillWs prefill_ws(const HostStep *steps, int n, int64_t M) {
 size_t prefill_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) { return prefill_ws(steps, n, M).end; }
 
 // Per step two launches: the pre-pass with the step's x op as a plain launch (it reads what the previous GEMM wrote and
-// overwrites the operand that GEMM read), then the GEMM with PDL as in gemm_forward.
+// overwrites the operand that GEMM read; one launch rotates x for every partition, where per-partition rotate_kernel launches
+// cost 3 x ~7 us at 256 tokens), then the GEMM with PDL.  A single linear above 16 rows runs as a one-step chain.
 int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
   const PrefillWs w = prefill_ws(steps, n, M);
   if (workspace_bytes < w.end) { set_error("workspace too small: have %zu, need %zu", workspace_bytes, w.end); return PARO_EWORKSPACE; }
@@ -468,7 +435,7 @@ int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspa
 int gemm_grouped_launch(const Layout &L, const void *packed, long long expert_stride, const void *xr, void *y, int NT, int slots,
                         const int32_t *rows, const int32_t *tile_expert, const int32_t *live_tiles, int dtype, cudaStream_t stream) {
   GemmParams p = {};
-  fill_weights(p, L);
+  p.L = L;
   p.packed = static_cast<const uint8_t *>(packed);
   p.xr = static_cast<const uint8_t *>(xr);
   p.y = y;

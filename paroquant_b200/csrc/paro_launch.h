@@ -16,13 +16,11 @@ int rotate_launch(const void *x, void *out, const int16_t *idx, const void *thet
 int rotate_backward_launch(const void *y, const void *gout, const void *x, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
                            int scales_dtype, void *grad_x, float *grad_theta, float *grad_scale, int64_t M, int K, int krot, int G, int dtype,
                            int ref_formula, cudaStream_t stream);
-// the pre-pass of the tensor-core kernels: x [M, K] rotated for every partition of L, M_store rows per partition (rows >= M zero)
-// in the B-operand order of tiles of nt tokens
-int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream);
 int rotate_routed_launch(const Layout &L, const void *packed, bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles,
                          int top_k, void *out, int rows_max, int nt, cudaStream_t stream);
-// the same pre-pass after a chain step's x op (PARO_XOP_*): NONE reads x [M, K]; SILU_MUL x [M, 2K] (gate | up); RMSNORM
-// h = x [M, K] with norm_w [K] and the producing step's fp32 sums of h^2, stats[b * M + m] for its 128-column blocks b < stats_blocks
+// the pre-pass of the tensor-core kernels: x rotated for every partition of L, M_store rows per partition (rows >= M zero) in the
+// B-operand order of tiles of nt tokens, after a chain step's x op (PARO_XOP_*): NONE reads x [M, K]; SILU_MUL x [M, 2K] (gate | up);
+// RMSNORM h = x [M, K] with norm_w [K] and the producing step's fp32 sums of h^2, stats[b * M + m] for its 128-column blocks b < stats_blocks
 int rotate_chain_launch(const Layout &L, const void *packed, int x_op, const void *x, const void *norm_w, const float *stats, int stats_blocks,
                         float eps, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream);
 
@@ -46,16 +44,12 @@ size_t stream_sync_bytes(const Layout &L);
 size_t stream_workspace_bytes(const Layout &L, int64_t max_m);
 size_t stream_chain_workspace_bytes(const HostStep *steps, int n, int64_t M);
 int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream);
-int stream_linear_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M, const void *bias, void *y,
-                          void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int stream_trace_read(unsigned long long *host, int max_ctas);
 int stream_debug_plan(const Layout &L, int64_t M, int sets, int ctas, int32_t *out);
 
 // paro_gemm.cu
 size_t gemm_workspace_bytes(const Layout &L, int64_t max_m);
 int gemm_debug_plan(const Layout &L, int64_t M, int sms, int32_t *out);
-int gemm_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M,
-                 const void *bias, void *y, void *workspace, size_t workspace_bytes, cudaStream_t stream);
 int gemm_grouped_launch(const Layout &L, const void *packed, long long expert_stride, const void *xr, void *y, int NT, int slots,
                         const int32_t *rows, const int32_t *tile_expert, const int32_t *live_tiles, int dtype, cudaStream_t stream);
 // a chain for any M (paro_prefill_chain_forward): per step the pre-pass with the step's x op, then the GEMM with its epilogue

@@ -64,14 +64,18 @@ PARO_HD constexpr int meta_pairs_off(int r) { return r * 128; }
 PARO_HD constexpr int meta_theta_off(int krot, int r) { return krot * 128 + r * 128; }
 PARO_HD constexpr int meta_scales_off(int krot) { return krot * 256; }
 
+// Every kernel's parameters carry one.  The field order sets which ints ptxas loads from the parameter bank in pairs: this one
+// keeps decode_kernel at 78 registers.
 struct Layout {
-  int K, N, krot, n_parts, dtype;
+  int K, N, n_parts;
   int groups;                               // K / 128: 128-channel record groups (each holds `qhalves` quantisation groups)
-  int qhalves, rec_bytes;                   // group_size 128: 1, 8576;  group_size 64: 2, 8960
+  int krot;
+  int meta_group_bytes;                     // krot*256 + 256
+  int rec_bytes, qhalves;                   // group_size 128: 8576, 1;  group_size 64: 8960, 2
   int blocks_total;                         // sum over partitions of ceil(size / 128)
+  int dtype;
   int part_col_begin[PARO_MAX_PARTS + 1];   // first output column of each partition
   int part_block_begin[PARO_MAX_PARTS + 1]; // cumulative blocks per partition
-  int meta_group_bytes;                     // krot*256 + 256
   size_t meta_off, rec_off, total_bytes;
 
   PARO_HD size_t meta_offset(int part, int gk) const {

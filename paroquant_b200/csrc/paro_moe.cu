@@ -50,10 +50,8 @@ struct MoeParams {
   void *y;                      // launch 1: h [T, k, N]; launch 2: out [T, N]
   const int32_t *ids;
   const float *wts;
-  int T, k, E, K, N;
-  int groups, krot, rec_bytes, q2, meta_group_bytes;
-  long long meta_off, rec_off;
-  int part_col_begin[3], part_block_begin[3];   // gate_up: 2 partitions; down: 1
+  int T, k, E;
+  Layout L;                     // one expert's linear (gate_up: 2 partitions; down: 1)
   int c, S, nstages;
   int xb_off, rot_off, recv_off, tab_off, bar_off;
 };
@@ -85,9 +83,9 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
   int *s_uexp = s_ids + kMoeMaxEntries;
   int *s_first = s_uexp + kMoeMaxEntries;
   uint32_t *s_mask = reinterpret_cast<uint32_t *>(s_first + kMoeMaxEntries);   // [u][16 tokens]: slots of token t that chose u
-  const int NS = p.nstages, c = p.c, S = p.S, G = p.groups;
+  const int NS = p.nstages, c = p.c, S = p.S, G = p.L.groups;
   const int b = blockIdx.x / c, rank = blockIdx.x - b * c;   // rank == %cluster_ctarank
-  const uint32_t rec_bytes = static_cast<uint32_t>(p.rec_bytes);
+  const uint32_t rec_bytes = static_cast<uint32_t>(p.L.rec_bytes);
 
   if (warp == kMoeWorkers) {
     ring_init(bar_wfull, bar_wempty, NS, kMoeWorkers, lane);
@@ -137,7 +135,7 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
       if (i < nitems) {
         int u, g0, g1;
         moe_item(i, S, G, u, g0, g1);
-        const uint8_t *src = p.packed + s_uexp[u] * p.stride + p.rec_off + (static_cast<size_t>(b) * G + g0) * rec_bytes;
+        const uint8_t *src = p.packed + s_uexp[u] * p.stride + p.L.rec_off + (static_cast<size_t>(b) * G + g0) * rec_bytes;
 #pragma unroll 1
         for (int g = g0; g < g1; ++g) {
           prod.issue([src] { return src; }, rec_bytes, pol, [] {});
@@ -154,14 +152,14 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
   // ================= workers
   const int tile = warp & 7, kh = warp >> 3;
   const int g = lane >> 2, t4 = lane & 3;
-  const RoundLane lo = round_lane<kMoeN>(p.q2 != 0, tile, kh, lane);
+  const RoundLane lo = round_lane<kMoeN>(p.L.qhalves == 2, tile, kh, lane);
   // the ring position persists across items and waves; a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * rec_bytes
   RingCursor rg = {bar_wfull, 0u, bar_wfull, bar_wfull + 8 * NS, 8 * kMoeMaxStages, rec_bytes / 8, smem0 - bar_wfull * (rec_bytes / 8), rec_bytes};
   const int ntok = p.T, nel = ntok * kBlockN;
   float yacc[4] = {0.f, 0.f, 0.f, 0.f}, oacc[4] = {0.f, 0.f, 0.f, 0.f};   // rank 0: elements tid + 512 q = (token, column)
   // my output columns (launch 1: gate_up has two partitions; a last partial block is masked at the stores)
-  const int part = b >= p.part_block_begin[1] ? 1 : 0;
-  const int n0 = p.part_col_begin[part] + (b - p.part_block_begin[part]) * kBlockN, n_end = p.part_col_begin[part + 1];
+  const int part = b >= p.L.part_block_begin[1] ? 1 : 0;
+  const int n0 = p.L.part_col_begin[part] + (b - p.L.part_block_begin[part]) * kBlockN, n_end = p.L.part_col_begin[part + 1];
   cluster_wait_acquire();   // phase 0: every CTA of the cluster runs
 
 #pragma unroll 1
@@ -176,10 +174,10 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
       const int R = __popc(tokmask);
       // ---- B operand of the item: zero rows [R, 16), then the rotation tasks (group x block of up to 4 rows) of the expert's
       // rows: its tokens (`tokmask`) ascending.  Launch 1 reads x[t]; launch 2 reads h[t, first slot of t] and applies SiLU * up.
-      const uint8_t *meta = p.packed + s_uexp[u] * p.stride + p.meta_off;   // partition 0 (gate and up share it)
+      const uint8_t *meta = p.packed + s_uexp[u] * p.stride + p.L.meta_off;   // partition 0 (gate and up share it)
       const int nq = R > 4 ? (R + 3) >> 2 : 1, ntasks = ng * nq;
       RotMeta rm;
-      if (warp < ntasks) fetch_meta<false>(meta + static_cast<size_t>(g0 + warp / nq) * p.meta_group_bytes, p.krot, lane, rm);
+      if (warp < ntasks) fetch_meta<false>(meta + static_cast<size_t>(g0 + warp / nq) * p.L.meta_group_bytes, p.L.krot, lane, rm);
       for (int idx = tid; idx < ng * (kMoeN * 16); idx += 32 * kMoeWorkers) sts128u(xb + idx * 16, make_uint4(0u, 0u, 0u, 0u));
       named_bar_sync(1, 32 * kMoeWorkers);
       {
@@ -195,21 +193,21 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
               const int t = nth_bit(tokmask, m0 + j);
               if constexpr (DOWN) {
                 const int slot = __ffs(umask[t]) - 1;   // duplicate slots of one token carry the same h row
-                const T *row = static_cast<const T *>(p.x) + (static_cast<int64_t>(t) * p.k + slot) * (2 * p.K) + gk * kGroup + 4 * lane;
-                const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + p.K));
+                const T *row = static_cast<const T *>(p.x) + (static_cast<int64_t>(t) * p.k + slot) * (2 * p.L.K) + gk * kGroup + 4 * lane;
+                const uint2 gate = __ldcg(reinterpret_cast<const uint2 *>(row)), up = __ldcg(reinterpret_cast<const uint2 *>(row + p.L.K));
                 raw[j].x = silu_mul2<T>(gate.x, up.x);
                 raw[j].y = silu_mul2<T>(gate.y, up.y);
               } else {
-                raw[j] = __ldcg(reinterpret_cast<const uint2 *>(static_cast<const T *>(p.x) + static_cast<int64_t>(t) * p.K + gk * kGroup + 4 * lane));
+                raw[j] = __ldcg(reinterpret_cast<const uint2 *>(static_cast<const T *>(p.x) + static_cast<int64_t>(t) * p.L.K + gk * kGroup + 4 * lane));
               }
             }
           }
           scale_and_stage<T, ROWS>(rot, lane, raw, csw);
         };
-        const int mg = p.meta_group_bytes;
-        if (R == 1) rotation_tasks<T, 1, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
-        else if (R == 2) rotation_tasks<T, 2, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
-        else rotation_tasks<T, 4, false>(rm, meta, mg, p.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
+        const int mg = p.L.meta_group_bytes;
+        if (R == 1) rotation_tasks<T, 1, false>(rm, meta, mg, p.L.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
+        else if (R == 2) rotation_tasks<T, 2, false>(rm, meta, mg, p.L.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
+        else rotation_tasks<T, 4, false>(rm, meta, mg, p.L.krot, g0, ntasks, nq, R, warp, kMoeWorkers, lane, rot, xb, kMoeN, stage_x);
       }
       named_bar_sync(2, 32 * kMoeWorkers);   // B operand complete
       // ---- rounds: the item is one segment of the round loop
@@ -258,7 +256,7 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
                 } else {
                   const int nn = n0 + col;
                   if (nn < n_end)
-                    for (uint32_t mm = m; mm; mm &= mm - 1) static_cast<T *>(p.y)[(static_cast<int64_t>(t) * p.k + __ffs(mm) - 1) * p.N + nn] = v;
+                    for (uint32_t mm = m; mm; mm &= mm - 1) static_cast<T *>(p.y)[(static_cast<int64_t>(t) * p.k + __ffs(mm) - 1) * p.L.N + nn] = v;
                 }
               }
               yacc[q] = 0.f;
@@ -273,7 +271,7 @@ __global__ void __launch_bounds__(kMoeThreads, 1) moe_kernel(const MoeParams p) 
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int e = tid + 32 * kMoeWorkers * q;
-        if (e < nel && n0 + (e & 127) < n_end) static_cast<T *>(p.y)[static_cast<int64_t>(e >> 7) * p.N + n0 + (e & 127)] = Traits<T>::from_float(oacc[q]);
+        if (e < nel && n0 + (e & 127) < n_end) static_cast<T *>(p.y)[static_cast<int64_t>(e >> 7) * p.L.N + n0 + (e & 127)] = Traits<T>::from_float(oacc[q]);
       }
     }
   }
@@ -362,13 +360,7 @@ static int moe_check(const paro_moe_desc *d, int64_t T, int32_t k, MoeShapes &ms
 static void moe_fill(MoeParams &p, const Layout &L, const MoePlan &m, const void *packed, size_t stride) {
   p.packed = static_cast<const uint8_t *>(packed);
   p.stride = static_cast<long long>(stride);
-  p.K = L.K; p.N = L.N;
-  p.groups = L.groups; p.krot = L.krot; p.rec_bytes = L.rec_bytes; p.q2 = L.qhalves == 2; p.meta_group_bytes = L.meta_group_bytes;
-  p.meta_off = static_cast<long long>(L.meta_off); p.rec_off = static_cast<long long>(L.rec_off);
-  for (int i = 0; i < 3; ++i) {
-    p.part_col_begin[i] = L.part_col_begin[i];
-    p.part_block_begin[i] = L.part_block_begin[i];
-  }
+  p.L = L;
   p.c = m.c; p.S = m.S; p.nstages = m.nstages;
   p.xb_off = m.xb_off; p.rot_off = m.rot_off; p.recv_off = m.recv_off; p.tab_off = m.tab_off; p.bar_off = m.bar_off;
 }

@@ -416,13 +416,6 @@ static int rotate_small_rows(const Layout &L, const void *packed, const Rows &sr
   return PARO_OK;
 }
 
-int rotate_small_launch(const Layout &L, const void *packed, const void *x, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {
-  if (L.dtype == PARO_F16)
-    return rotate_small_rows<__half>(L, packed, DenseRows<__half>{static_cast<const __half *>(x), static_cast<int>(M), L.K}, out, M_store, nt, stream);
-  return rotate_small_rows<__nv_bfloat16>(L, packed, DenseRows<__nv_bfloat16>{static_cast<const __nv_bfloat16 *>(x), static_cast<int>(M), L.K}, out,
-                                          M_store, nt, stream);
-}
-
 template <typename T>
 static int rotate_chain_T(const Layout &L, const void *packed, int x_op, const void *x, const void *norm_w, const float *stats, int stats_blocks,
                           float eps, void *out, int64_t M, int64_t M_store, int nt, cudaStream_t stream) {

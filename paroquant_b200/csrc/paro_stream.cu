@@ -79,12 +79,8 @@ struct StepDesc {
   int x_op, epi_op;
   int stats_in_blocks;
   int x_ld;
-  int K, N, n_parts, groups, krot, meta_group_bytes;
-  int rec_bytes, q2;        // record size; q2: group_size 64, two scale / zero sets per record (paro_layout.h)
-  int c, T, max_slots, blocks_total;
-  long long meta_off, rec_off;
-  int part_col_begin[PARO_MAX_PARTS + 1];
-  int part_block_begin[PARO_MAX_PARTS + 1];
+  Layout L;                 // the packed linear (paro_layout.h)
+  int c, T, max_slots;
   int part_cta_begin[PARO_MAX_PARTS + 1];   // members u of a slice (u = cta / c) dealt to the partitions
 };
 
@@ -98,6 +94,7 @@ struct StreamParams {
   uint32_t *sync;             // [0] epoch (tag of a launch = epoch + 1), [1] CTAs done
   StepDesc steps[kStmMaxSteps];
 };
+static_assert(sizeof(StreamParams) <= 4096, "kernel parameters are limited to 4 KB");
 
 // ---- where a CTA works in a step
 struct StepGeom {
@@ -116,9 +113,9 @@ __device__ __forceinline__ StepGeom step_geom(const StepDesc &S, int cta) {
   g.part = part;
   g.t = u - S.part_cta_begin[part];
   g.Tp = S.part_cta_begin[part + 1] - S.part_cta_begin[part];
-  g.g_begin = static_cast<int>(static_cast<unsigned>(g.slice * S.groups) / static_cast<unsigned>(S.c));
-  g.ng = static_cast<int>(static_cast<unsigned>((g.slice + 1) * S.groups) / static_cast<unsigned>(S.c)) - g.g_begin;
-  g.blocks_p = S.part_block_begin[part + 1] - S.part_block_begin[part];
+  g.g_begin = static_cast<int>(static_cast<unsigned>(g.slice * S.L.groups) / static_cast<unsigned>(S.c));
+  g.ng = static_cast<int>(static_cast<unsigned>((g.slice + 1) * S.L.groups) / static_cast<unsigned>(S.c)) - g.g_begin;
+  g.blocks_p = S.L.part_block_begin[part + 1] - S.L.part_block_begin[part];
   // 32-bit on purpose (a 64-bit division is a ~150-instruction subroutine on the GPU): the host checks Rp * Tp < 2^31
   const unsigned Rp = static_cast<unsigned>(g.blocks_p * g.ng), Tp = static_cast<unsigned>(g.Tp);
   g.r0 = static_cast<int>(static_cast<unsigned>(g.t) * Rp / Tp);
@@ -273,7 +270,7 @@ __device__ __forceinline__ void stm_rstd(const StepDesc &S, int M, int lane, uin
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
-    if (lane == 0) sts_f32(rstd_smem + 4 * m, rsqrtf(s / static_cast<float>(S.K) + S.eps));
+    if (lane == 0) sts_f32(rstd_smem + 4 * m, rsqrtf(s / static_cast<float>(S.L.K) + S.eps));
   }
 }
 
@@ -305,7 +302,7 @@ __device__ __forceinline__ void stm_load_x(const StepDesc &S, int M, int gk, int
           const uint4 *src = reinterpret_cast<const uint4 *>(S.x_ll + static_cast<int64_t>(m0 + m) * S.x_ld + col);
           ok = ll_unpack4(ld_relaxed_v4(src), ld_relaxed_v4(src + 1), tag, raw[m]) && ok;
           if (silu) {
-            const uint4 *su = reinterpret_cast<const uint4 *>(S.x_ll + static_cast<int64_t>(m0 + m) * S.x_ld + S.K + col);
+            const uint4 *su = reinterpret_cast<const uint4 *>(S.x_ll + static_cast<int64_t>(m0 + m) * S.x_ld + S.L.K + col);
             ok = ll_unpack4(ld_relaxed_v4(su), ld_relaxed_v4(su + 1), tag, up[m]) && ok;
           }
         }
@@ -320,7 +317,7 @@ __device__ __forceinline__ void stm_load_x(const StepDesc &S, int M, int gk, int
       up[m] = make_uint2(0u, 0u);
       if (m0 + m < M) {
         raw[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * S.x_ld));
-        if (silu) up[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * S.x_ld + S.K));
+        if (silu) up[m] = __ldcg(reinterpret_cast<const uint2 *>(xg + static_cast<int64_t>(m0 + m) * S.x_ld + S.L.K));
       }
     }
   }
@@ -388,8 +385,8 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       const StepDesc &S = p.steps[i];
       const StepGeom g = step_geom(S, cta);
       if (!g.active) continue;
-      const uint32_t rec_bytes = static_cast<uint32_t>(S.rec_bytes);
-      const uint8_t *rec_part = S.packed + S.rec_off + (static_cast<size_t>(S.part_block_begin[g.part]) * S.groups + g.g_begin) * rec_bytes;
+      const uint32_t rec_bytes = static_cast<uint32_t>(S.L.rec_bytes);
+      const uint8_t *rec_part = S.packed + S.L.rec_off + (static_cast<size_t>(S.L.part_block_begin[g.part]) * S.L.groups + g.g_begin) * rec_bytes;
       const SegWalk sw = seg_walk(g);
 #pragma unroll 1
       for (int k = 0; k < sw.nseg; ++k) {
@@ -401,7 +398,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
         for (int r = ra; r < rb; ++r, ++gi) {
           // at most `inflight` records outstanding per SM (the stage of copy n - inflight has not been reused yet)
           if (issued >= static_cast<uint32_t>(p.inflight)) mbar_wait(bar_wfull + 8 * lag_st, lag_it & 1);
-          prod.issue([=, &S] { return rec_part + (static_cast<size_t>(jb) * S.groups + gi) * rec_bytes; }, rec_bytes, pol, [] {});
+          prod.issue([=, &S] { return rec_part + (static_cast<size_t>(jb) * S.L.groups + gi) * rec_bytes; }, rec_bytes, pol, [] {});
           if (++issued > static_cast<uint32_t>(p.inflight)) {
             if (++lag_st == NS) { lag_st = 0; ++lag_it; }
           }
@@ -424,7 +421,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       const StepDesc &S = p.steps[i];
       const StepGeom g = step_geom(S, cta);
       if (!g.active) continue;
-      const int n_end = S.part_col_begin[g.part + 1];
+      const int n_end = S.L.part_col_begin[g.part + 1];
       const SegWalk sw = seg_walk(g);
       const bool tp = S.tp_world > 1;
       // Every segment's accumulator goes to its slot as soon as it completes -- nothing ever waits before that, so
@@ -441,11 +438,11 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
         int ra, rb;
         seg_range(sw, k, ra, rb);
         const int jb = static_cast<int>(static_cast<unsigned>(ra) / static_cast<unsigned>(g.ng));
-        const int gb = S.part_block_begin[g.part] + jb;
+        const int gb = S.L.part_block_begin[g.part] + jb;
         int total = 0, myslot = 0;
         unsigned gs0 = 0;
         for (int sl = 0; sl < S.c; ++sl) {
-          const unsigned gs1 = static_cast<unsigned>((sl + 1) * S.groups) / static_cast<unsigned>(S.c);
+          const unsigned gs1 = static_cast<unsigned>((sl + 1) * S.L.groups) / static_cast<unsigned>(S.c);
           const int ngs = static_cast<int>(gs1 - gs0);
           gs0 = gs1;
           const int Rp = g.blocks_p * ngs;
@@ -476,7 +473,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       auto sum_block = [&](int gb, int total, unsigned long long bit, float (&acc)[MB]) -> bool {
         const bool pushed = (pushed_mask & bit) != 0ull;
         if (S.epi_op == PARO_EPI_ADD_RESIDUAL) {   // warm the residual lines this block's finish will read (they sit in L2)
-          const int n = S.part_col_begin[g.part] + (gb - S.part_block_begin[g.part]) * kBlockN + L128;
+          const int n = S.L.part_col_begin[g.part] + (gb - S.L.part_block_begin[g.part]) * kBlockN + L128;
           if (n < n_end) asm volatile("prefetch.global.L2 [%0];" ::"l"(static_cast<const T *>(S.res_in) + n));
         }
         if (!pushed) {
@@ -488,7 +485,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
           // my block sum goes to every rank (mine included), then the `world` sums are added in rank order -- every rank
           // computes the same bits.  Nothing waits before the push.  Buffers alternate with the launch parity: a rank that
           // is one launch ahead writes the other half while this one is still reading.
-          const size_t blk = (static_cast<size_t>(tag & 1u) * S.blocks_total + gb) * S.tp_world;
+          const size_t blk = (static_cast<size_t>(tag & 1u) * S.L.blocks_total + gb) * S.tp_world;
           if (!pushed) {
             for (int rk = 0; rk < S.tp_world; ++rk) {
               uint2 *dst = S.tp_slots[rk] + (blk + S.tp_rank) * (M * 128) + L128;
@@ -508,7 +505,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       // round once to T, bias, epilogue, publish for the next step
       auto finish_block = [&](int jb, int gb, float (&acc)[MB]) {
         if (warp == kEpiWarp0) STM_TRACE(i, 9);
-        const int n = S.part_col_begin[g.part] + jb * kBlockN + L128;
+        const int n = S.L.part_col_begin[g.part] + jb * kBlockN + L128;
         const bool ok = n < n_end;
         const bool add_res = S.epi_op == PARO_EPI_ADD_RESIDUAL;
 #pragma unroll
@@ -517,7 +514,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
           if (m < M && ok) {
             T t = Traits<T>::from_float(acc[m]);
             if (S.bias) t = Traits<T>::from_float(Traits<T>::to_float(t) + Traits<T>::to_float(static_cast<const T *>(S.bias)[n]));  // plugin.py:309-310
-            const int64_t o = static_cast<int64_t>(m) * S.N + n;
+            const int64_t o = static_cast<int64_t>(m) * S.L.N + n;
             if (S.y) static_cast<T *>(S.y)[o] = t;
             if (add_res) {
               t = Traits<T>::from_float(Traits<T>::to_float(t) + Traits<T>::to_float(static_cast<const T *>(S.res_in)[o]));
@@ -625,7 +622,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       const int ntasks = g.active ? g.ng * nq : 0;
       const bool mine = wi < ntasks && wi < p.rot_warps;
       RotMeta rm;
-      if (mine) fetch_meta(S.packed + S.meta_off + (static_cast<size_t>(g.part) * S.groups + g.g_begin + wi / nq) * S.meta_group_bytes, S.krot, lane, rm);   // flies during the waits below
+      if (mine) fetch_meta(S.packed + S.L.meta_off + (static_cast<size_t>(g.part) * S.L.groups + g.g_begin + wi / nq) * S.L.meta_group_bytes, S.L.krot, lane, rm);   // flies during the waits below
       if (i == 0) {
         // rows [M, NR) of every group are zero padding of the MMA's N: cleared once (M is the same for every step)
         if (M < NR) {
@@ -652,15 +649,15 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
           stm_load_x<T>(S, M, g.g_begin + gi, lane, raw, m0, tag, rstd_smem);
           scale_and_stage<T>(rot, lane, raw, csw);
         };
-        const uint8_t *meta = S.packed + S.meta_off;
-        const int mi0 = g.part * S.groups + g.g_begin, mg = S.meta_group_bytes, rw = p.rot_warps;
+        const uint8_t *meta = S.packed + S.L.meta_off;
+        const int mi0 = g.part * S.L.groups + g.g_begin, mg = S.L.meta_group_bytes, rw = p.rot_warps;
         if constexpr (MB == 1) {
-          rotation_tasks<T, 1, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
+          rotation_tasks<T, 1, true>(rm, meta, mg, S.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         } else if constexpr (MB == 4) {
-          if (M == 2) rotation_tasks<T, 2, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
-          else rotation_tasks<T, 4, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
+          if (M == 2) rotation_tasks<T, 2, true>(rm, meta, mg, S.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
+          else rotation_tasks<T, 4, true>(rm, meta, mg, S.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         } else {
-          rotation_tasks<T, 4, true>(rm, meta, mg, S.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
+          rotation_tasks<T, 4, true>(rm, meta, mg, S.L.krot, mi0, ntasks, nq, M, wi, rw, lane, rot, xb, NR, stage_x);
         }
       }
       named_bar_sync(2, 32 * kWorkers);   // B operand of this step complete
@@ -678,7 +675,7 @@ __global__ void __launch_bounds__(32 * (4 * SETS + 5), 1) stream_kernel(const __
       // never wraps.  A segment starting at an odd stage takes its first record alone, an odd remainder its last.
       auto segments = [&](auto ntt, auto nr) {
         constexpr int NTT = decltype(ntt)::value, NRC = decltype(nr)::value;
-        const RoundLane lo = round_lane<NRC>(S.q2 != 0, tile, kh, lane);
+        const RoundLane lo = round_lane<NRC>(S.L.qhalves == 2, tile, kh, lane);
         const uint32_t ring_end = bar_wfull + 8 * NS, stage_bytes = p.stage_bytes;
         // a stage's record from its full barrier: smem0 + (fb - bar_wfull) / 8 * stage_bytes (a multiple of 8)
         const uint32_t rec_per_bar = stage_bytes / 8, rec_at_bar0 = smem0 - bar_wfull * rec_per_bar;
@@ -893,8 +890,8 @@ static int stm_launch(StreamParams &p, int max_ng, int ctas, cudaStream_t stream
   PARO_CUDA_OK(smem_opt_in(kern, kStmSmemLimit));
   if (kn.verbose) {
     for (int i = 0; i < p.n_steps; ++i)
-      fprintf(stderr, "[paro stream] step %d K=%d N=%d M=%d: %d slices x %d members, <= %d slots/block, xop %d epi %d wait %d\n", i, p.steps[i].K,
-              p.steps[i].N, M, p.steps[i].c, p.steps[i].T, p.steps[i].max_slots, p.steps[i].x_op, p.steps[i].epi_op, p.steps[i].x_ll ? 1 : 0);
+      fprintf(stderr, "[paro stream] step %d K=%d N=%d M=%d: %d slices x %d members, <= %d slots/block, xop %d epi %d wait %d\n", i, p.steps[i].L.K,
+              p.steps[i].L.N, M, p.steps[i].c, p.steps[i].T, p.steps[i].max_slots, p.steps[i].x_op, p.steps[i].epi_op, p.steps[i].x_ll ? 1 : 0);
     fprintf(stderr, "[paro stream] %d CTAs, %d stages, B rows %d, rot warps %d, smem %d\n", ctas, p.nstages, p.nrows_b, p.rot_warps, smem_total);
   }
   cudaLaunchConfig_t cfg;
@@ -951,17 +948,10 @@ int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, siz
     S.stats_ll = consumed && h.epi_op == PARO_EPI_ADD_RESIDUAL ? reinterpret_cast<uint2 *>(ws + w.stats_off) : nullptr;
     S.out_ll = consumed ? reinterpret_cast<uint2 *>(ws + w.out_off) : nullptr;
     S.slots = reinterpret_cast<uint2 *>(ws + w.slots_off);
-    S.K = L.K; S.N = L.N; S.n_parts = L.n_parts; S.groups = L.groups; S.krot = L.krot; S.meta_group_bytes = L.meta_group_bytes;
-    S.c = pl.c; S.T = pl.T; S.max_slots = pl.max_slots; S.blocks_total = L.blocks_total;
-    S.meta_off = static_cast<long long>(L.meta_off);
-    S.rec_off = static_cast<long long>(L.rec_off);
-    S.rec_bytes = L.rec_bytes; S.q2 = L.qhalves == 2;
+    S.L = L;
+    S.c = pl.c; S.T = pl.T; S.max_slots = pl.max_slots;
     if (L.rec_bytes > p.stage_bytes) p.stage_bytes = L.rec_bytes;
-    for (int k = 0; k <= PARO_MAX_PARTS; ++k) {
-      S.part_col_begin[k] = L.part_col_begin[k];
-      S.part_block_begin[k] = L.part_block_begin[k];
-      S.part_cta_begin[k] = pl.part_cta_begin[k];
-    }
+    for (int k = 0; k <= PARO_MAX_PARTS; ++k) S.part_cta_begin[k] = pl.part_cta_begin[k];
     if (h.tp && h.tp->world > 1) {
       S.tp_world = h.tp->world;
       S.tp_rank = h.tp->rank;
@@ -974,7 +964,7 @@ int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, siz
       const StepDesc &P = p.steps[i - 1];
       S.x_ll = P.out_ll;
       S.stats_in = P.stats_ll;
-      S.stats_in_blocks = 4 * P.blocks_total;   // one partial sum per (block, epilogue warp)
+      S.stats_in_blocks = 4 * P.L.blocks_total;   // one partial sum per (block, epilogue warp)
     }
     if (pl.ng_max > max_ng) max_ng = pl.ng_max;
   }
@@ -982,17 +972,6 @@ int stream_forward(const HostStep *steps, int n, int64_t M, void *workspace, siz
   if (p.M == 1) return bf16 ? stm_launch<__nv_bfloat16, kStmSets, 1>(p, max_ng, sms, stream) : stm_launch<__half, kStmSets, 1>(p, max_ng, sms, stream);
   if (p.M <= 4) return bf16 ? stm_launch<__nv_bfloat16, kStmSets, 4>(p, max_ng, sms, stream) : stm_launch<__half, kStmSets, 4>(p, max_ng, sms, stream);
   return bf16 ? stm_launch<__nv_bfloat16, kStmSets, 16>(p, max_ng, sms, stream) : stm_launch<__half, kStmSets, 16>(p, max_ng, sms, stream);
-}
-
-// single linear (paro_linear_forward, M <= 16)
-int stream_linear_forward(const paro_linear_shape &s, const Layout &L, const void *packed, const void *x, int64_t M, const void *bias, void *y,
-                          void *workspace, size_t workspace_bytes, cudaStream_t stream) {
-  HostStep h = {};
-  h.shape = &s;
-  h.L = L;
-  h.packed = packed; h.bias = bias; h.x = x; h.y = y;
-  h.x_op = PARO_XOP_NONE; h.epi_op = PARO_EPI_STORE;
-  return stream_forward(&h, 1, M, workspace, workspace_bytes, stream);
 }
 
 }  // namespace paro
