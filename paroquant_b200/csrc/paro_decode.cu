@@ -445,7 +445,7 @@ static int launch_decode(DecParams &p, const DecCached &c, cudaStream_t stream) 
 
 bool decode_supported(const Layout &L, int64_t M) { return M >= 1 && M <= 16 && L.groups >= 1; }
 
-// From 5 rows on (3 when K >= 8192) the rotation runs ONCE, in a pre-pass (paro_rotate.cu: rotate_small_kernel, one launch for all
+// From 5 rows on (3 when K >= 8192) the rotation runs ONCE, in a pre-pass (paro_rotate.cu: rotate_tile_kernel, one launch for all
 // partitions, ~2.5 us) that writes x_rot in this kernel's B-operand order, and the kernel fetches its K slice with one bulk copy.
 // Inside the kernel a 4-row rotation task is ~1000 dependent instructions of one warp (7-14 k cycles with 20 warps contending) and
 // at M = 16 a CTA has 32-56 of them: 28 k of o_proj's 40 k cycles, 48 k of down_proj's 80 k (tools/trace_decode.py).  Measured
@@ -474,7 +474,7 @@ int decode_forward(const paro_linear_shape &s, const Layout &L, const void *pack
   if (!found) { set_error("decode: no launch configuration fits (in_features=%d, M=%d)", L.K, static_cast<int>(M)); return PARO_EUNSUPPORTED; }
   const size_t part_bytes = static_cast<size_t>(kDecN) * L.K * 2;   // 16 rows (zero padded) x K of T, B-operand order
   const bool prerot = decode_wants_prerot(L, M) && scratch && scratch_bytes >= L.n_parts * part_bytes;
-  if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_small_kernel)
+  if (prerot) {   // one launch for all partitions (paro_rotate.cu: rotate_tile_kernel)
     const int rc = rotate_chain_launch(L, packed, PARO_XOP_NONE, x, nullptr, nullptr, 0, 0.f, scratch, M, kDecN, kDecN, stream);
     if (rc) return rc;
   }

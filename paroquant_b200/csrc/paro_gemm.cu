@@ -393,7 +393,7 @@ static PrefillWs prefill_ws(const HostStep *steps, int n, int64_t M) {
 size_t prefill_chain_workspace_bytes(const HostStep *steps, int n, int64_t M) { return prefill_ws(steps, n, M).end; }
 
 // Per step two launches: the pre-pass with the step's x op as a plain launch (it reads what the previous GEMM wrote and
-// overwrites the operand that GEMM read; one launch rotates x for every partition, where per-partition rotate_kernel launches
+// overwrites the operand that GEMM read; one launch rotates x for every partition, where one rotate launch per partition
 // cost 3 x ~7 us at 256 tokens), then the GEMM with PDL.  A single linear above 16 rows runs as a one-step chain.
 int prefill_chain_forward(const HostStep *steps, int n, int64_t M, void *workspace, size_t workspace_bytes, cudaStream_t stream) {
   const PrefillWs w = prefill_ws(steps, n, M);

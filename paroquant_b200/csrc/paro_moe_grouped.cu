@@ -9,7 +9,7 @@
 //   1. route     one CTA: counts the valid entries (t, s) of every expert, gives each expert a run of NT-row tiles and writes
 //                the routing table -- the entries sorted by (expert, token, slot), each expert's run padded with -1 to a
 //                whole tile, the expert of every tile and the live tile count.  Rewritten in full every launch.
-//   2. pre-pass  rotate_small_kernel (paro_rotate.cu) with a gather row source: x[t] of every table position, rotated by the
+//   2. pre-pass  rotate_tile_kernel (paro_rotate.cu) with a gather row source: x[t] of every table position, rotated by the
 //                block's gate_up rotation, straight into the B-operand tile order of the GEMM; padding rows zero.
 //   3. GEMM      wg_gemm_kernel (paro_gemm.cu) with the grouped tile source: CTA = (tile slot, 128-column block), the weights
 //                of the tile's expert, the epilogue scatters row (t, s) to h[t, s].  Slots past the live count exit at once.

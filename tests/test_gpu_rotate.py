@@ -248,7 +248,7 @@ PREPASS_CASES = [
 
 @pytest.mark.parametrize("K,parts,M,G,krot,dt", PREPASS_CASES)
 def test_prepass_operand_is_the_rotate_op_bit_for_bit(ops, K, parts, M, G, krot, dt):
-    """The tensor-core kernels' pre-pass (rotate_small_kernel, reading the packed layout's metadata blocks) writes, for every
+    """The tensor-core kernels' pre-pass (rotate_tile_kernel, reading the packed layout's metadata blocks) writes, for every
     partition, exactly torch.ops.rotation.rotate of the same rows in the B-operand tile order, padding rows zero."""
     import ctypes
     from paroquant_b200 import _cabi

@@ -18,6 +18,11 @@ from paroquant_b200 import _cabi  # noqa: E402
 from paroquant_b200.checkpoint import make_synthetic_layer  # noqa: E402
 
 
+# (dtype, M, K, group): the training shapes, also the forward column of tools/rotate_op_bench.py
+SHAPES = ((torch.float32, 4096, 4096, 128), (torch.bfloat16, 4096, 4096, 128), (torch.float32, 14336, 4096, 128),
+          (torch.float32, 4096, 4096, 64), (torch.float32, 256, 4096, 128))
+
+
 def stagewise(x, idx_ij, theta, y, grad_out, scale, G):
     krot, K = idx_ij.shape
     rows = y.numel() // K
@@ -52,8 +57,7 @@ if __name__ == "__main__":
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     res = []
-    for dt, M, K, G in ((torch.float32, 4096, 4096, 128), (torch.bfloat16, 4096, 4096, 128), (torch.float32, 14336, 4096, 128),
-                        (torch.float32, 4096, 4096, 64), (torch.float32, 256, 4096, 128)):
+    for dt, M, K, G in SHAPES:
         L = make_synthetic_layer(K, [64], group_size=G, seed=5, device="cuda")
         pr, th, sc = L.pairs[0], L.theta[0].float(), L.channel_scales[0].float().view(-1)
         x = torch.randn(M, K, device="cuda").to(dt)
