@@ -106,6 +106,13 @@ int paro_rotate_backward(const void *y, const void *grad_out, const void *x, con
                          int32_t krot, int32_t group_size, int32_t dtype, int32_t theta_formula,
                          paro_stream_t stream);
 
+/* Test hook (host only, no device work): the launch plan of paro_rotate_backward on a device with `sms` SMs, the function the
+ * launch itself uses.  out[0] = dynamic shared-memory bytes per CTA, out[1] = CTAs per SM it plans for, out[2] = splits (warps
+ * per group; warp `split` walks row blocks split, split + splits, ...), out[3] = row blocks of 4 rows, out[4] / out[5] = the
+ * most / fewest row blocks one warp walks, out[6] = grid CTAs.  M >= 1; the other arguments as paro_rotate_backward takes them. */
+int paro_debug_rotate_backward_plan(int64_t M, int32_t K, int32_t krot, int32_t group_size, int32_t dtype,
+                                    int32_t theta_formula, int32_t sms, int64_t *out);
+
 /* Size in bytes of the kernel-layout buffer paro_prepack fills (0 on invalid shape). */
 size_t paro_packed_bytes(const paro_linear_shape *shape);
 

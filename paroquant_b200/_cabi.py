@@ -86,6 +86,8 @@ def lib() -> ctypes.CDLL:
         L.paro_rotate.argtypes = [vp, vp, vp, vp, i32, vp, i32, i64, i32, i32, i32, i32, vp]
         L.paro_rotate_backward.restype = ctypes.c_int
         L.paro_rotate_backward.argtypes = [vp, vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp]
+        L.paro_debug_rotate_backward_plan.restype = ctypes.c_int
+        L.paro_debug_rotate_backward_plan.argtypes = [i64, i32, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_int64)]
         L.paro_packed_bytes.restype = sz
         L.paro_packed_bytes.argtypes = [shp]
         L.paro_prepack.restype = ctypes.c_int
@@ -146,6 +148,7 @@ EXPORTED_SYMBOLS = (
     "paro_debug_gemm_plan", "paro_moe_workspace_bytes", "paro_moe_forward", "paro_debug_moe_plan", "paro_debug_silu_mul",
     "paro_moe_grouped_workspace_bytes", "paro_moe_grouped_forward", "paro_debug_moe_grouped_plan",
     "paro_prefill_chain_workspace_bytes", "paro_prefill_chain_forward", "paro_moe_route", "paro_debug_moe_route_plan",
+    "paro_debug_rotate_backward_plan",
 )
 
 
@@ -249,6 +252,21 @@ def rotate_backward(y: torch.Tensor, grad_out: torch.Tensor, x: torch.Tensor, id
                                         dtype_code(y.dtype), 1 if reference_formula else 0, _stream(dev))
     _check(rc, "rotate_backward")
     return grad_x, grad_theta, grad_scale
+
+
+ROTATE_BACKWARD_PLAN_FIELDS = ("dyn_smem", "ctas_per_sm", "splits", "row_blocks", "max_blocks_per_warp", "min_blocks_per_warp", "grid")
+
+
+def debug_rotate_backward_plan(M: int, K: int, krot: int, group_size: int, dtype: torch.dtype, reference_formula: bool = False,
+                               sms: int | None = None) -> dict:
+    """paro_debug_rotate_backward_plan: the launch plan `rotate_backward` uses, as a dict of ROTATE_BACKWARD_PLAN_FIELDS (host
+    only; sms defaults to cuda:0's SM count)."""
+    if sms is None:
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+    out = (ctypes.c_int64 * len(ROTATE_BACKWARD_PLAN_FIELDS))()
+    _check(lib().paro_debug_rotate_backward_plan(M, K, krot, group_size, dtype_code(dtype), 1 if reference_formula else 0, sms, out),
+           "debug_rotate_backward_plan")
+    return dict(zip(ROTATE_BACKWARD_PLAN_FIELDS, out))
 
 
 def packed_bytes(shape: ParoLinearShape) -> int:

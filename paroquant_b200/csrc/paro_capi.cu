@@ -143,6 +143,17 @@ int paro_rotate_backward(const void *y, const void *grad_out, const void *x, con
                                 dtype, theta_formula, static_cast<cudaStream_t>(stream));
 }
 
+int paro_debug_rotate_backward_plan(int64_t M, int32_t K, int32_t krot, int32_t group_size, int32_t dtype, int32_t theta_formula, int32_t sms,
+                                    int64_t *out) {
+  if (!out || sms < 1 || M < 1) { set_error("debug_rotate_backward_plan: bad arguments"); return PARO_EINVAL; }
+  if (theta_formula != PARO_THETA_GRADIENT && theta_formula != PARO_THETA_REFERENCE_EXPRESSION) { set_error("rotate_backward: unknown theta_formula %d", theta_formula); return PARO_EINVAL; }
+  if (!valid_dtype(dtype)) { set_error("rotate supports Float, Half, and BFloat16, got dtype code %d", dtype); return PARO_EINVAL; }
+  if (group_size != 64 && group_size != 128) { set_error("Unsupported group_size: %d; expected 64 or 128", group_size); return PARO_EUNSUPPORTED; }
+  if (K <= 0 || K % group_size) { set_error("h must be divisible by GROUP_SIZE"); return PARO_EINVAL; }
+  if (krot < 1 || krot > 16) { set_error("Unsupported KROT = %d; supported: 1..16", krot); return PARO_EUNSUPPORTED; }
+  return rotate_backward_debug_plan(M, K, krot, group_size, theta_formula, sms, out);
+}
+
 size_t paro_packed_bytes(const paro_linear_shape *shape) {
   Layout L;
   if (!layout_of(shape, "packed_bytes", L)) return 0;

@@ -16,6 +16,7 @@ int rotate_launch(const void *x, void *out, const int16_t *idx, const void *thet
 int rotate_backward_launch(const void *y, const void *gout, const void *x, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
                            int scales_dtype, void *grad_x, float *grad_theta, float *grad_scale, int64_t M, int K, int krot, int G, int dtype,
                            int ref_formula, cudaStream_t stream);
+int rotate_backward_debug_plan(int64_t M, int K, int krot, int G, int ref_formula, int sms, int64_t *out);
 int rotate_routed_launch(const Layout &L, const void *packed, bool silu_mul, const void *src, const int32_t *rows, const int32_t *live_tiles,
                          int top_k, void *out, int rows_max, int nt, cudaStream_t stream);
 // the pre-pass of the tensor-core kernels: x rotated for every partition of L, M_store rows per partition (rows >= M zero) in the

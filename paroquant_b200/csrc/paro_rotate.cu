@@ -603,24 +603,51 @@ __global__ void __launch_bounds__(128) rotate_backward_kernel(const T *__restric
   }
 }
 
+// The backward's launch plan, pure host logic (paro_debug_rotate_backward_plan drives it without a GPU).  Per CTA: 4 warps x krot
+// x G/2 pairs x ({cos, sin} 8 B + slots 4 B + partial 4 B) of dynamic shared memory (+ 4 B: the g . t sums of the reference's
+// expression) next to the two static tiles; as many CTAs per SM as that leaves room for, at most 6 (the register limit).  Enough
+// (split, group) warps to fill the machine, no more splits than row blocks: every warp then walks ~row_blocks / splits blocks of
+// its group (split, split + splits, ...), computes the group's (cos, sin) once and pays its atomics once.
+struct BackwardPlan {
+  size_t dyn;
+  int ctas_per_sm;
+  int64_t row_blocks, splits, blocks;
+};
+static BackwardPlan backward_plan(int64_t M, int K, int krot, int G, int ref_formula, int sms) {
+  BackwardPlan p;
+  const int groups = K / G;
+  p.row_blocks = (M + 3) / 4;
+  p.dyn = static_cast<size_t>(4) * krot * (G / 2) * (ref_formula ? 20 : 16);
+  const int resident = static_cast<int>((227 * 1024) / (p.dyn + static_cast<size_t>(8) * G * 16 + 1024));
+  p.ctas_per_sm = resident < 1 ? 1 : resident > 6 ? 6 : resident;
+  p.splits = (static_cast<int64_t>(sms) * p.ctas_per_sm * 4 + groups - 1) / groups;
+  if (p.splits > p.row_blocks) p.splits = p.row_blocks;
+  if (p.splits < 1) p.splits = 1;
+  p.blocks = (p.splits * groups + 3) / 4;
+  return p;
+}
+
+int rotate_backward_debug_plan(int64_t M, int K, int krot, int G, int ref_formula, int sms, int64_t *out) {
+  const BackwardPlan p = backward_plan(M, K, krot, G, ref_formula, sms);
+  out[0] = static_cast<int64_t>(p.dyn);
+  out[1] = p.ctas_per_sm;
+  out[2] = p.splits;
+  out[3] = p.row_blocks;
+  out[4] = (p.row_blocks + p.splits - 1) / p.splits;   // the most row blocks a warp walks
+  out[5] = p.row_blocks / p.splits;                    // the fewest
+  out[6] = p.blocks;
+  return PARO_OK;
+}
+
 template <typename T>
 static int launch_backward_T(const void *y, const void *gout, const void *x, const int16_t *idx, const void *theta, int theta_dtype, const void *scales,
                              int scales_dtype, void *grad_x, float *grad_theta, float *grad_scale, int64_t M, int K, int krot, int G, int ref_formula,
                              cudaStream_t stream) {
-  const int groups = K / G;
-  const int64_t row_blocks = (M + 3) / 4;
-  // per CTA: 4 warps x krot x G/2 pairs x ({cos, sin} 8 B + slots 4 B + partial 4 B) of dynamic shared memory + the two tiles
-  const size_t dyn = static_cast<size_t>(4) * krot * (G / 2) * (ref_formula ? 20 : 16);   // (+ 4 B: the g . t sums of the reference's expression)
-  const int resident = static_cast<int>((227 * 1024) / (dyn + static_cast<size_t>(8) * G * 16 + 1024));
-  const int ctas_per_sm = resident < 1 ? 1 : resident > 6 ? 6 : resident;   // 6: the register limit
-  // enough warps to fill the machine, no more splits than row blocks: every warp then walks ~row_blocks / splits blocks of its
-  // group, computes the group's (cos, sin) once and pays its atomics once
   const int sms = device_sms();
   if (sms <= 0) { set_error("rotate_backward: no CUDA device"); return PARO_ECUDA; }
-  int64_t splits = (static_cast<int64_t>(sms) * ctas_per_sm * 4 + groups - 1) / groups;
-  if (splits > row_blocks) splits = row_blocks;
-  if (splits < 1) splits = 1;
-  const int64_t blocks = (splits * groups + 3) / 4;
+  const BackwardPlan plan = backward_plan(M, K, krot, G, ref_formula, sms);
+  const size_t dyn = plan.dyn;
+  const int64_t splits = plan.splits, blocks = plan.blocks;
   if (blocks > 0x7FFFFFFF) { set_error("rotate_backward: too many groups"); return PARO_EINVAL; }
   const T *yp = static_cast<const T *>(y), *gp = static_cast<const T *>(gout), *xp = static_cast<const T *>(x);
   T *gx = static_cast<T *>(grad_x);

@@ -392,3 +392,125 @@ def check_moe(y: torch.Tensor, h: torch.Tensor, ids: torch.Tensor, w: torch.Tens
         tok, ws = [torch.zeros(0, dtype=torch.long, device=dev)], [torch.zeros(0, device=dev)]
         ys = mag = [torch.zeros(0, N, dtype=torch.float64, device=dev)]
     return check_combine(y, torch.cat(tok), torch.cat(ws), torch.cat(ys), torch.cat(mag), what)
+
+
+# ---- the rotate op's backward (paro_rotate_backward)
+U32 = 2.0 ** -24                  # fp32 unit roundoff
+FTZ_PER_ROW = 2.0 ** -125         # the kernel flushes fp32 subnormals: two flushed products of at most 2^-126 each per row
+_F64_SUM = 2.0 ** -52             # torch's fp64 row sums of exact products, per row (far below one fp32 step)
+
+
+def backward_restated(x: torch.Tensor, pairs: torch.Tensor, theta: torch.Tensor, y: torch.Tensor, grad_out: torch.Tensor,
+                      scales: torch.Tensor | None, group: int) -> dict:
+    """The rotate op's backward restated, for x, y = rotate(x), grad_out [M, K] in T on the GPU.  The stage values come from
+    the reference's walk (autograd.py:20-61): from rotation krot - 1 down to 0, t and g are un-rotated by one-rotation rotate-op
+    launches with -theta, which round them to T where the fused kernel does (the rotate op equals `exact_rotate` value for value).
+    Every product of two stage values, or of x and g, is a product of fp32 values and so exact in fp64.  Returns, on y's device:
+
+      grad_x      T(fp32(g * scale as stored)) (g without scales), [M, K] in T
+      S, D        per rotation and pair, sum_rows (g_i t_j - g_j t_i) and sum_rows (g_i t_i + g_j t_j) in fp64, [krot, K / 2]
+      A, B        their magnitudes sum_rows |g_i t_j| + |g_j t_i| and sum_rows |g_i t_i| + |g_j t_j|
+      xg, xg_abs  sum_rows x g and sum_rows |x g| per channel in fp64, [K] (None without scales)
+
+    The pair slots are group-relative, as the op takes them."""
+    import paroquant_b200.kernels.cuda  # noqa: F401  registers torch.ops.rotation.rotate
+    krot, K = pairs.shape
+    rows = y.numel() // K
+    t, g = y.reshape(rows, K).contiguous(), grad_out.reshape(rows, K).contiguous()
+    base = (torch.arange(K, device=y.device) // group * group).view(K // 2, 2)[:, 0]
+    out = {k: torch.zeros(krot, K // 2, dtype=torch.float64, device=y.device) for k in "SDAB"}
+    for r in reversed(range(krot)):
+        pr = pairs[r].view(K // 2, 2).long()
+        ci, cj = pr[:, 0] + base, pr[:, 1] + base
+        gi, gj, ti, tj = g[:, ci].double(), g[:, cj].double(), t[:, ci].double(), t[:, cj].double()
+        a, b, c, d = gi * tj, gj * ti, gi * ti, gj * tj
+        out["S"][r], out["D"][r] = (a - b).sum(0), (c + d).sum(0)
+        out["A"][r], out["B"][r] = (a.abs() + b.abs()).sum(0), (c.abs() + d.abs()).sum(0)
+        del gi, gj, ti, tj, a, b, c, d
+        inv = -theta[r:r + 1]
+        t = torch.ops.rotation.rotate(t, pairs[r:r + 1], inv, None, group)
+        g = torch.ops.rotation.rotate(g, pairs[r:r + 1], inv, None, group)
+    if scales is None:
+        out["grad_x"], out["xg"], out["xg_abs"] = g, None, None
+    else:
+        out["grad_x"] = (g.float() * scales.float().reshape(-1)).to(y.dtype)
+        xg = x.reshape(rows, K).double() * g.double()
+        out["xg"], out["xg_abs"] = xg.sum(0), xg.abs().sum(0)
+    out["rows"] = rows
+    return out
+
+
+def backward_depths(max_blocks: int, splits: int) -> tuple[int, int]:
+    """The fp32 steps a term of the backward's row sums goes through, for a plan whose warps walk at most `max_blocks` row blocks
+    of 4 rows and whose `splits` warp partials per entry are added with fp32 atomics (paro_debug_rotate_backward_plan).
+    grad_theta: 2 for the product difference, 3 within a 4-row block, one per block in the warp's running sum, one per atomic.
+    grad_scale: 1 for the product, one per row in the warp's running sum (4 per block), one per atomic."""
+    return 5 + max_blocks + splits, 1 + 4 * max_blocks + splits
+
+
+def _gamma(d: int) -> float:
+    return d * U32 / (1 - d * U32)
+
+
+def _assert_entries(got: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, keep: torch.Tensor, label, what: str, show: int) -> float:
+    err = (got.double() - ref).abs()
+    bad = keep & ~(err <= tol)                                # NaN / inf in got count as violations
+    if bool(bad.any()):
+        idx = bad.nonzero().tolist()
+        lines = [f"  ({label(*i)}): got {float(got[tuple(i)]):.9g} ref {float(ref[tuple(i)]):.9g} tol {float(tol[tuple(i)]):.3g}"
+                 for i in idx[:show]]
+        raise AssertionError(f"{what}: {len(idx)} of {int(keep.sum())} entries outside the element-wise bound\n" + "\n".join(lines))
+    return float((err[keep] / tol[keep]).max()) if bool(keep.any()) else 0.0
+
+
+def check_backward_theta(got: torch.Tensor, ref: dict, c: torch.Tensor, s: torch.Tensor, group: int, max_blocks: int, splits: int,
+                         reference_formula: bool = False, skip_groups=(), cast: torch.dtype | None = None, what: str = "",
+                         show: int = 6) -> float:
+    """grad_theta [krot, K / 2] of the fused backward against `backward_restated`'s sums.  With d = backward_depths(...)[0] and
+    M rows, every entry must satisfy
+
+        gradient:              |got - S| <= gamma_d A + 2^-125 M
+        reference expression:  |got - (c S + s D)| <= gamma_(d+2) (|c| A + |s| B) + 2^-124 M
+
+    (gamma_d = d u / (1 - d u), u = 2^-24; the M terms cover flushed subnormal products and, far below them, the fp64 sums).
+    (c, s) [krot, K / 2] is the kernel's own __sincosf(-T(theta)) (`kernel_sincos`); the expression's two extra steps are its
+    product and sum.  cast: the dtype grad_theta was cast to after the sum (autograd returns it in theta's dtype): one more
+    rounding, ulp_cast(got).  Entries of `skip_groups` are not checked; every other entry must be finite.  Raises AssertionError
+    naming the violating entries as (rotation, group, pair) with got / ref / tol; returns the largest err / tol."""
+    dev = ref["S"].device
+    d = backward_depths(max_blocks, splits)[0]
+    rows = ref["rows"]
+    if reference_formula:
+        cd, sd = c.to(dev).double(), s.to(dev).double()
+        exact = cd * ref["S"] + sd * ref["D"]
+        tol = _gamma(d + 2) * (cd.abs() * ref["A"] + sd.abs() * ref["B"]) + 2 * FTZ_PER_ROW * rows
+    else:
+        exact = ref["S"]
+        tol = _gamma(d) * ref["A"] + FTZ_PER_ROW * rows
+    tol = tol + _F64_SUM * rows * (ref["A"] + ref["B"])
+    got = got.to(dev)
+    if cast is not None:
+        tol = tol + ulp(got, cast)
+    per = group // 2
+    keep = torch.ones_like(exact, dtype=torch.bool)
+    for gr in skip_groups:
+        keep[:, gr * per:(gr + 1) * per] = False
+    return _assert_entries(got, exact, tol, keep, lambda r, p: f"rotation {r}, group {p // per}, pair {p % per}", what, show)
+
+
+def check_backward_scale(got: torch.Tensor, ref: dict, group: int, max_blocks: int, splits: int, skip_groups=(),
+                         cast: torch.dtype | None = None, what: str = "", show: int = 6) -> float:
+    """grad_scale [K] of the fused backward against `backward_restated`'s sum_rows x g: with d = backward_depths(...)[1],
+    |got - xg| <= gamma_d xg_abs + 2^-125 M per channel (cast, skip_groups as `check_backward_theta`).  Raises AssertionError
+    naming the violating channels with got / ref / tol; returns the largest err / tol."""
+    dev = ref["xg"].device
+    rows = ref["rows"]
+    d = backward_depths(max_blocks, splits)[1]
+    tol = _gamma(d) * ref["xg_abs"] + FTZ_PER_ROW * rows + _F64_SUM * rows * ref["xg_abs"]
+    got = got.to(dev).reshape(-1)
+    if cast is not None:
+        tol = tol + ulp(got, cast)
+    keep = torch.ones_like(tol, dtype=torch.bool)
+    for gr in skip_groups:
+        keep[gr * group:(gr + 1) * group] = False
+    return _assert_entries(got, ref["xg"], tol, keep, lambda ch: f"channel {ch}, group {ch // group}", what, show)

@@ -16,6 +16,7 @@ import torch
 from paroquant_b200.checkpoint import make_synthetic_activations, make_synthetic_layer
 
 from conftest import GOLDEN
+from gpu_reference import backward_restated
 
 pytestmark = pytest.mark.gpu
 _TD = {"float32": torch.float32, "float16": torch.float16, "bfloat16": torch.bfloat16}
@@ -144,28 +145,9 @@ def test_autograd_matches_dense_jacobian(ops):
         assert (a - b).norm() / b.norm() < 2e-5
 
 
-def _backward_stagewise(x, idx_ij, theta, y, grad_out, scale, G):
-    """The reference's backward structure (kernels/cuda/autograd.py:20-61): walk the rotations last to first with one-rotation
-    rotate launches on t and g; test-side restatement the fused backward kernel is compared with."""
-    krot, K = idx_ij.shape
-    rows = y.numel() // K
-    t, g = y.reshape(rows, K), grad_out.reshape(rows, K).contiguous()
-    base = (torch.arange(K, device=idx_ij.device) // G * G).view(K // 2, 2)[:, 0]
-    grad_theta = torch.zeros(krot, K // 2, dtype=torch.float32, device=y.device)
-    for r in reversed(range(krot)):
-        pr = idx_ij[r].view(K // 2, 2).long()
-        ci, cj = pr[:, 0] + base, pr[:, 1] + base
-        grad_theta[r] = (g[:, ci].float() * t[:, cj].float() - g[:, cj].float() * t[:, ci].float()).sum(0)
-        inv = -theta[r:r + 1]
-        t = torch.ops.rotation.rotate(t, idx_ij[r:r + 1], inv, None, G)
-        g = torch.ops.rotation.rotate(g, idx_ij[r:r + 1], inv, None, G)
-    if scale is None:
-        return g.view_as(x), grad_theta, None
-    return (g.float() * scale.float().reshape(-1)).to(x.dtype).view_as(x), grad_theta, (x.reshape(rows, K).float() * g.float()).sum(0)
-
-
 @pytest.mark.parametrize("dt,G,krot,M,with_scale", [
-    (torch.float32, 128, 8, 1037, True),       # many row blocks per warp, ragged last block
+    (torch.float32, 128, 8, 1037, True),       # ragged last block; at K 1024 every warp walks one row block (multi-block sums:
+                                               # tests/test_gpu_rotate_backward.py)
     (torch.float32, 64, 8, 333, True),
     (torch.float32, 128, 3, 5, False),         # no channel scales, krot != 8
     (torch.bfloat16, 128, 8, 260, True),       # t and g rounded to bf16 after every rotation, like the per-rotation launches
@@ -181,7 +163,8 @@ def test_fused_backward_equals_the_stagewise_walk(ops, dt, G, krot, M, with_scal
     go = torch.randn(M, K, device="cuda").to(dt)
     y = torch.ops.rotation.rotate(x, pr, th, sc, G)
     gx, gth, gsc = _cabi.rotate_backward(y, go, x, pr, th, sc, G)
-    rx, rth, rsc = _backward_stagewise(x, pr, th, y, go, sc, G)
+    R = backward_restated(x, pr, th, y, go, sc, G)    # the reference's walk: one-rotation rotate launches with -theta
+    rx, rth, rsc = R["grad_x"], R["S"], R["xg"]
     # grad_x: the same arithmetic at the same rounding points -> identical
     assert torch.equal(gx, rx)
     # row sums: fp32 atomics in another order than torch's reduction

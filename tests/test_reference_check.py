@@ -2,12 +2,14 @@
 flags a single element that normwise relative error 1e-3 lets through (a 64-channel partial sum missing, or 3 ulps off).
 `check_combine` (a MoE block's weighted sum of expert outputs) accepts any fp32 order of the expert sums and of the slot
 combine, and flags faults of the block's reduction and combine that the oracle comparisons' normwise and per-row bounds let
-through."""
+through.  `check_backward_theta` / `check_backward_scale` (the rotate op's fused backward) accept the kernel's fp32 sums taken
+over rows in any order, in 4-row blocks, per warp and across warps by atomics in any order, and flag a block missing or counted
+twice, a pair's term from its neighbour and two rotations' sums swapped."""
 import pytest
 import torch
 
-from gpu_reference import (_nudge, check, check_combine, check_residual, check_rmsnorm, exact_bias, exact_rms_rows, linear_bound,
-                           rms_candidates, rms_operand, ulp)
+from gpu_reference import (_nudge, backward_depths, check, check_backward_scale, check_backward_theta, check_combine, check_residual,
+                           check_rmsnorm, exact_bias, exact_rms_rows, linear_bound, rms_candidates, rms_operand, ulp)
 
 M, K, PARTS = 32, 4096, [1024, 1024]
 
@@ -399,3 +401,215 @@ def test_residual_bound_flags_one_block_of_one_row(dt):
     assert _rel(bad, h) < 1e-3
     with pytest.raises(AssertionError, match=rf"elements outside the element-wise bound\n.*\(row {m}, col \d+, block {b}, part 0\)"):
         check_residual(bad, t, r)
+
+
+# ---- the rotate op's fused backward: grad_theta and grad_scale
+BG, BK, BKROT, BM = 128, 256, 3, 2003                     # 2 groups; 501 row blocks, the last one ragged
+
+
+def _bwd_case(seed=0):
+    """Stage values t_r, g_r [krot, M, K] (fp32, independent per rotation: the bound does not care where they come from), x, the
+    absolute pair channels [krot, K / 2] of random group-relative pairs, (c, s) of random angles, and the fp64 sums of
+    `backward_restated`."""
+    g = torch.Generator().manual_seed(seed)
+    t = torch.randn(BKROT, BM, BK, generator=g)
+    gr = torch.randn(BKROT, BM, BK, generator=g) * 0.01
+    x = torch.randn(BM, BK, generator=g)
+    base = (torch.arange(BK) // BG * BG).view(BK // 2, 2)[:, 0]
+    ci, cj = [], []
+    for _ in range(BKROT):
+        perm = torch.cat([torch.randperm(BG, generator=g) + q * BG for q in range(BK // BG)]).view(BK // 2, 2) - base[:, None]
+        ci.append(perm[:, 0] + base)
+        cj.append(perm[:, 1] + base)
+    ci, cj = torch.stack(ci), torch.stack(cj)
+    ang = (torch.rand(BKROT, BK // 2, generator=g) * 2 - 1) * 3.0
+    c, s = ang.cos(), ang.sin()
+    ref = {k: torch.zeros(BKROT, BK // 2, dtype=torch.float64) for k in "SDAB"}
+    for r in range(BKROT):
+        gi, gj, ti, tj = (v.double() for v in (gr[r][:, ci[r]], gr[r][:, cj[r]], t[r][:, ci[r]], t[r][:, cj[r]]))
+        a, b, cc, d = gi * tj, gj * ti, gi * ti, gj * tj
+        ref["S"][r], ref["D"][r], ref["A"][r], ref["B"][r] = (a - b).sum(0), (cc + d).sum(0), (a.abs() + b.abs()).sum(0), (cc.abs() + d.abs()).sum(0)
+    xg = x.double() * gr[0].double()                      # grad_scale: x times the last un-rotated g
+    ref["xg"], ref["xg_abs"], ref["rows"] = xg.sum(0), xg.abs().sum(0), BM
+    return t, gr, x, ci, cj, c, s, ref
+
+
+def _warp_sums(rows_terms, splits, block_sum, fault=None):
+    """The kernel's per-warp fp32 running sums: rows_terms [M, E] fp32 -> [splits, E].  Row blocks of 4 (zero rows pad the last),
+    block b summed by block_sum([4, E]) and added to warp b % splits in block order.  fault: ("drop" | "twice", block)."""
+    M, E = rows_terms.shape
+    rb = (M + 3) // 4
+    nb = (rb + splits - 1) // splits
+    padded = torch.zeros(nb * splits * 4, E)
+    padded[:M] = rows_terms
+    blocks = padded.view(nb, splits, 4, E)
+    acc = torch.zeros(splits, E)
+    for i in range(nb):
+        for w in range(splits):
+            b = i * splits + w
+            if fault == ("drop", b):
+                continue
+            part = block_sum(blocks[i, w])
+            acc[w] = acc[w] + part
+            if fault == ("twice", b):
+                acc[w] = acc[w] + part
+    return acc
+
+
+def _atomics(parts, g):
+    """fp32 atomics of the warp partials [splits, E] into a zeroed buffer, in a random order."""
+    out = torch.zeros(parts.shape[1])
+    for w in torch.randperm(parts.shape[0], generator=g).tolist():
+        out = out + parts[w]
+    return out
+
+
+def _theta_rows(t, gr, ci, cj, r):
+    gi, gj, ti, tj = gr[r][:, ci[r]], gr[r][:, cj[r]], t[r][:, ci[r]], t[r][:, cj[r]]
+    return gi * tj - gj * ti, gi * ti + gj * tj            # fp32: two products and a difference per row
+
+
+def _block4(v):
+    return ((v[0] + v[1]) + v[2]) + v[3]
+
+
+def _kernel_like_theta(case, splits, seed, reference_formula=False, fault=None, rotation=None):
+    """grad_theta [krot, K / 2] summed as the kernel does, rows taken in a random order (fault applied in rotation `rotation`, or
+    all rotations when None: a block a warp drops or repeats is dropped or repeated for all its entries)."""
+    t, gr, x, ci, cj, c, s, ref = case
+    g = torch.Generator().manual_seed(seed)
+    perm = torch.randperm(BM, generator=g)
+    out = torch.zeros(BKROT, BK // 2)
+    for r in range(BKROT):
+        f = fault if rotation in (None, r) else None
+        cross, dot = (v[perm] for v in _theta_rows(t, gr, ci, cj, r))
+        acc = _warp_sums(cross, splits, _block4, f)
+        if reference_formula:
+            acc = c[r] * acc + s[r] * _warp_sums(dot, splits, _block4, f)
+        out[r] = _atomics(acc, g)
+    return out
+
+
+def _kernel_like_scale(case, splits, seed, fault=None):
+    t, gr, x, ci, cj, c, s, ref = case
+    g = torch.Generator().manual_seed(seed)
+    perm = torch.randperm(BM, generator=g)
+    prods = (x * gr[0])[perm]                              # acc_s += x * g row by row: one fp32 step per row
+    M, E = prods.shape
+    rb = (M + 3) // 4
+    nb = (rb + splits - 1) // splits
+    padded = torch.zeros(nb * splits * 4, E)
+    padded[:M] = prods
+    blocks = padded.view(nb, splits, 4, E)
+    acc = torch.zeros(splits, E)
+    for i in range(nb):
+        for w in range(splits):
+            b = i * splits + w
+            reps = 0 if fault == ("drop", b) else 2 if fault == ("twice", b) else 1
+            for _ in range(reps):
+                for q in range(4):
+                    acc[w] = acc[w] + blocks[i, w, q]
+    return _atomics(acc, g)
+
+
+def _plan_depth(splits):
+    rb = (BM + 3) // 4
+    return (rb + splits - 1) // splits, splits
+
+
+@pytest.mark.parametrize("splits", [1, 7, 66, 251, 501])
+@pytest.mark.parametrize("reference_formula", [False, True])
+def test_backward_bounds_accept_any_row_order_and_atomic_order(splits, reference_formula):
+    case = _bwd_case()
+    c, s, ref = case[5], case[6], case[7]
+    nb, sp = _plan_depth(splits)
+    for seed in (1, 2):
+        got = _kernel_like_theta(case, splits, seed, reference_formula)
+        assert check_backward_theta(got, ref, c, s, BG, nb, sp, reference_formula, what=f"splits {splits}") <= 1.0
+        assert check_backward_scale(_kernel_like_scale(case, splits, seed), ref, BG, nb, sp) <= 1.0
+
+
+def test_backward_depths():
+    assert backward_depths(16, 66) == (5 + 16 + 66, 1 + 64 + 66)
+
+
+@pytest.mark.parametrize("fault", ["drop", "twice"])
+@pytest.mark.parametrize("reference_formula", [False, True])
+def test_backward_bound_flags_one_block_missing_or_duplicated_in_one_warp(fault, reference_formula):
+    case = _bwd_case(seed=3)
+    c, s, ref = case[5], case[6], case[7]
+    splits = 66
+    nb, sp = _plan_depth(splits)
+    blk = 66 * 4 + 67                                      # row block 331: warp 1 (group 0 in this layout of the rows), 6th block
+    got = _kernel_like_theta(case, splits, 5, reference_formula, fault=(fault, blk), rotation=1)
+    with pytest.raises(AssertionError, match=r"entries outside the element-wise bound\n.*\(rotation 1, group \d, pair \d+\)"):
+        check_backward_theta(got, ref, c, s, BG, nb, sp, reference_formula)
+    with pytest.raises(AssertionError, match=r"entries outside the element-wise bound\n.*\(channel \d+, group \d\)"):
+        check_backward_scale(_kernel_like_scale(case, splits, 5, fault=(fault, blk)), ref, BG, nb, sp)
+
+
+@pytest.mark.parametrize("reference_formula", [False, True])
+def test_backward_bound_flags_one_pair_from_its_neighbour(reference_formula):
+    case = _bwd_case(seed=4)
+    c, s, ref = case[5], case[6], case[7]
+    nb, sp = _plan_depth(66)
+    got = _kernel_like_theta(case, 66, 6, reference_formula)
+    assert check_backward_theta(got, ref, c, s, BG, nb, sp, reference_formula) <= 1.0
+    r, p = 2, 64 + 17                                      # group 1, pair 17 takes pair 18's sums
+    t, gr, x, ci, cj = case[:5]
+    ci2, cj2 = ci.clone(), cj.clone()
+    ci2[r, p], cj2[r, p] = ci[r, p + 1], cj[r, p + 1]
+    bad = _kernel_like_theta((t, gr, x, ci2, cj2, c, s, ref), 66, 6, reference_formula)
+    with pytest.raises(AssertionError, match=r"1 of 384 entries outside the element-wise bound\n  \(rotation 2, group 1, pair 17\)"):
+        check_backward_theta(bad, ref, c, s, BG, nb, sp, reference_formula)
+
+
+@pytest.mark.parametrize("reference_formula", [False, True])
+def test_backward_bound_flags_two_rotations_swapped(reference_formula):
+    case = _bwd_case(seed=5)
+    c, s, ref = case[5], case[6], case[7]
+    nb, sp = _plan_depth(7)
+    got = _kernel_like_theta(case, 7, 8, reference_formula)
+    bad = got.clone()
+    bad[[0, 1]] = got[[1, 0]]
+    with pytest.raises(AssertionError, match=r"entries outside the element-wise bound\n  \(rotation 0, group 0, pair \d+\)"):
+        check_backward_theta(bad, ref, c, s, BG, nb, sp, reference_formula)
+
+
+def test_backward_bound_skips_only_the_named_groups():
+    case = _bwd_case(seed=6)
+    c, s, ref = case[5], case[6], case[7]
+    nb, sp = _plan_depth(66)
+    got = _kernel_like_theta(case, 66, 9)
+    gsc = _kernel_like_scale(case, 66, 9)
+    got[:, 64 + 5], gsc[BG + 9] = float("nan"), float("inf")
+    assert check_backward_theta(got, ref, c, s, BG, nb, sp, skip_groups=[1]) <= 1.0
+    assert check_backward_scale(gsc, ref, BG, nb, sp, skip_groups=[1]) <= 1.0
+    with pytest.raises(AssertionError, match=r"3 of 384 entries.*\n  \(rotation 0, group 1, pair 5\): got nan"):
+        check_backward_theta(got, ref, c, s, BG, nb, sp)
+    with pytest.raises(AssertionError, match=r"1 of 128 entries.*\n  \(channel 137, group 1\): got inf"):
+        check_backward_scale(gsc, ref, BG, nb, sp, skip_groups=[0])
+
+
+def test_rotate_backward_plan_reaches_every_case_at_132_sms():
+    """paro_debug_rotate_backward_plan (the function the launch uses) on an H100 SXM's 132 SMs: every case of the GPU suite gets
+    the blocks per warp, the uneven split or the dynamic shared memory it is there for."""
+    from paroquant_b200 import _cabi
+    from rotate_backward_cases import CASES, assert_plan_reaches, case_id
+    for c in CASES:
+        dt, G, krot, M, K, forms, kind = c
+        for f in forms:
+            plan = _cabi.debug_rotate_backward_plan(M, K, krot, G, dt, f, sms=132)
+            assert_plan_reaches(plan, kind, M, f"{case_id(c)} reference_formula={f}")
+            assert plan["row_blocks"] == (M + 3) // 4
+            assert plan["grid"] == (plan["splits"] * (K // G) + 3) // 4
+    # the 48 KB opt-in: the krot-13 and krot-16 group-128 cases and the reference formula's krot 10, not krot 8
+    dyn = lambda krot, f=False: _cabi.debug_rotate_backward_plan(4096, 4096, krot, 128, torch.float32, f, sms=132)["dyn_smem"]
+    assert dyn(13) == 53248 and dyn(16) == 65536 and dyn(16, True) == 81920 and dyn(10, True) == 51200
+    assert dyn(8) <= 48 * 1024 and dyn(8, True) <= 48 * 1024 and dyn(12) <= 48 * 1024 and dyn(9, True) <= 48 * 1024
+    # what the old stage-wise cases (K 1024) got: one block per warp
+    for dt, G, krot, M in ((torch.float32, 128, 8, 1037), (torch.float32, 64, 8, 333), (torch.bfloat16, 128, 8, 260)):
+        assert _cabi.debug_rotate_backward_plan(M, 1024, krot, G, dt, sms=132)["max_blocks_per_warp"] == 1
+    for bad in ((0, 4096, 8, 128), (1, 4096, 17, 128), (1, 100, 8, 64), (1, 4096, 8, 32)):
+        with pytest.raises(RuntimeError, match="debug_rotate_backward_plan"):
+            _cabi.debug_rotate_backward_plan(*bad, torch.float32, sms=132)
